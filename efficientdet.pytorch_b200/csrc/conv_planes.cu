@@ -146,8 +146,7 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
-                    wg_mma3<NB, 0>(d, sa + k * 32, sa + kPlA + k * 32, sb + k * 32, sb + kPlB + k * 32, 64 * 128, 16, 1024,
-                                   (kt | k) != 0);
+                    wg_mma3<NB, 0>(d, sa + k * 32, sa + kPlA + k * 32, sb + k * 32, sb + kPlB + k * 32, 16, 1024, (kt | k) != 0);
                 wgmma_commit();
                 wgmma_wait<1>();                                   // the previous stage is no longer read
                 if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kPlStages]);

@@ -172,8 +172,7 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effd
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < kTileK / 16; ++k)
-                wg_mma3<NB, 0>(d, sa + k * 32, sa + S::kA + k * 32, sb + k * 32, sb + S::kB + k * 32, 64 * 128, 16, 1024,
-                               (kt | k) != 0);
+                wg_mma3<NB, 0>(d, sa + k * 32, sa + S::kA + k * 32, sb + k * 32, sb + S::kB + k * 32, 16, 1024, (kt | k) != 0);
             wgmma_commit();
         }
         wgmma_wait<0>();
@@ -354,7 +353,7 @@ wgrad_tc_kernel(const effdet_wgrad_args p, const int M, const int HW, const int 
     const int ch_end = min(nchunks, ch_begin + chunks_per_split);
     const int KT = ch_end - ch_begin;      // >= 1 by construction of the grid
     constexpr int NB = BC / 64;
-    constexpr uint32_t GROUP = kTileK * 128, SBO = 1024;
+    constexpr uint32_t GROUP = kTileK * 128;
     const int t = threadIdx.x, g = warp >> 2;      // warpgroup g: output channels n0 + 64g .. + 63
     float d[NB][32];
     for (int kt = 0; kt < KT; ++kt) {
@@ -369,12 +368,7 @@ wgrad_tc_kernel(const effdet_wgrad_args p, const int M, const int HW, const int 
         fence_proxy_async();
         named_bar_sync(1, kTcProducers);
         const uint32_t sa = smem_u32(a_hi) + g * GROUP, sb = smem_u32(b_hi);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kTileK / 16; ++k) {
-            const uint32_t ko = k * 2 * SBO;     // 16 pixels = two 8-row groups
-            wg_mma3<NB, 1>(d, sa + ko, sa + S::kA + ko, sb + ko, sb + S::kB + ko, GROUP, GROUP, SBO, (kt | k) != 0);
-        }
+        wg_mma3_mn_steps<kTileK / 16>(d, sa, sa + S::kA, sb, sb + S::kB, GROUP, kt != 0);
         wgmma_commit();
     }
     wgmma_wait<0>();
@@ -468,25 +462,21 @@ wgrad_tc2_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_consta
     } else {
         // two consumer warpgroups: wgmma on output channels n0 + 64 * wg .. + 63, then atomics into OIHW
         constexpr int NB = BC / 64;
-        constexpr uint32_t SBO = 1024;
         const int wg = warp >> 2;
-        const int ksteps = g.kstage / 16;
         float d[NB][32];
-        for (int kt = 0; kt < KT; ++kt) {
-            const int s = kt % STAGES;
-            const uint32_t ph = (kt / STAGES) & 1;
-            mbar_wait(&full_bar[s], ph);
-            const uint32_t sa = smem_u32(smem + s * S::kStage) + wg * GROUP;
-            const uint32_t sb = smem_u32(smem + s * S::kStage) + 2 * S::kA;
-            wgmma_fence();
-            for (int k = 0; k < ksteps; ++k) {
-                const uint32_t ko = k * 2 * SBO;
-                wg_mma3<NB, 1>(d, sa + ko, sa + S::kA + ko, sb + ko, sb + S::kB + ko, GROUP, GROUP, SBO, (kt | k) != 0);
+        with_count<1, 2, 3, 4>(g.kstage / 16, [&](auto ksteps) {
+            for (int kt = 0; kt < KT; ++kt) {
+                const int s = kt % STAGES;
+                const uint32_t ph = (kt / STAGES) & 1;
+                mbar_wait(&full_bar[s], ph);
+                const uint32_t sa = smem_u32(smem + s * S::kStage) + wg * GROUP;
+                const uint32_t sb = smem_u32(smem + s * S::kStage) + 2 * S::kA;
+                wg_mma3_mn_steps<ksteps>(d, sa, sa + S::kA, sb, sb + S::kB, GROUP, kt != 0);
+                wgmma_commit();
+                wgmma_wait<1>();                   // the previous stage is no longer read
+                if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % STAGES]);
             }
-            wgmma_commit();
-            wgmma_wait<1>();                       // the previous stage is no longer read
-            if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % STAGES]);
-        }
+        });
         wgmma_wait<0>();
         wg_atomic_dw<NB>(d, p.dw, n0 + 64 * wg, c0, p.Cout, p.Cin, p.ksize * p.ksize, tap);
     }
@@ -572,27 +562,24 @@ wgrad_tc2_multi_kernel(const __grid_constant__ WgMaps maps, const __grid_constan
         }
     } else {
         constexpr int NB = BC / 64;
-        constexpr uint32_t SBO = 1024;
         const int wg = warp >> 2;
-        int l = 0;
         float d[NB][32];
-        for (int kt = 0; kt < KT; ++kt) {
-            const int s = kt % STAGES;
-            const uint32_t ph = (kt / STAGES) & 1;
-            const int chg = ch_begin + kt;
-            while (l + 1 < a.nlevels && chg >= a.chunk_begin[l + 1]) ++l;
-            const int ksteps = __shfl_sync(0xffffffffu, a.g[l].kstage / 16, 0);   // warp-uniform by construction
-            mbar_wait(&full_bar[s], ph);
-            const uint32_t sa = smem_u32(smem + s * S::kStage) + wg * GROUP;
-            const uint32_t sb = smem_u32(smem + s * S::kStage) + 2 * S::kA;
-            wgmma_fence();
-            for (int k = 0; k < ksteps; ++k) {
-                const uint32_t ko = k * 2 * SBO;
-                wg_mma3<NB, 1>(d, sa + ko, sa + S::kA + ko, sb + ko, sb + S::kB + ko, GROUP, GROUP, SBO, (kt | k) != 0);
-            }
-            wgmma_commit();
-            wgmma_wait<1>();
-            if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % STAGES]);
+        // level by level: the pixel box, and so the number of K16 steps per stage, is fixed within a level
+        for (int kt = 0, l = 0; kt < KT; ++l) {
+            const int end = min(KT, a.chunk_begin[l + 1] - ch_begin);
+            with_count<1, 2, 3, 4>(a.g[l].kstage / 16, [&](auto ksteps) {
+                for (; kt < end; ++kt) {
+                    const int s = kt % STAGES;
+                    const uint32_t ph = (kt / STAGES) & 1;
+                    mbar_wait(&full_bar[s], ph);
+                    const uint32_t sa = smem_u32(smem + s * S::kStage) + wg * GROUP;
+                    const uint32_t sb = smem_u32(smem + s * S::kStage) + 2 * S::kA;
+                    wg_mma3_mn_steps<ksteps>(d, sa, sa + S::kA, sb, sb + S::kB, GROUP, kt != 0);
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % STAGES]);
+                }
+            });
         }
         wgmma_wait<0>();
         wg_atomic_dw<NB>(d, a.dw, n0 + 64 * wg, c0, a.Cout, a.Cin, a.ksize * a.ksize, tap);

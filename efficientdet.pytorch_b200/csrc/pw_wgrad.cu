@@ -197,27 +197,22 @@ __global__ void __launch_bounds__(kWgThreads, 1) pw_wgrad_kernel(const __grid_co
         // consumer warpgroup g: output channels n0 + 64g .. + 63.  A dy tile of at most 64 channels keeps ONE group in
         // shared memory; warpgroup 1 then multiplies the same group again and its rows are never stored.
         const int g = warp >> 2, w = warp & 3;
-        const uint32_t SBO = 1024;
         const uint32_t a_off = P.a_plane > group ? (uint32_t)(g * group) : 0u;
-        const int ksteps = P.K / 16;
         float d[NB][32];
-        for (int kt = 0; kt < KT; ++kt) {
-            const int s = kt % P.NS;
-            const uint32_t ph = (kt / P.NS) & 1;
-            mbar_wait(&full_bar[s], ph);
-            const uint32_t a_hi = smem_u32(smem + (size_t)s * P.stage_bytes) + a_off;
-            const uint32_t b_hi = smem_u32(smem + (size_t)s * P.stage_bytes) + 2 * P.a_plane;
-            wgmma_fence();
-            for (int k = 0; k < ksteps; ++k) {
-                const uint32_t ko = k * 2 * SBO;                 // 16 pixels = two 8-row groups
-                wg_mma3<NB, 1>(d, a_hi + ko, a_hi + P.a_plane + ko, b_hi + ko, b_hi + P.b_plane + ko, group, group, SBO,
-                               (kt | k) != 0);
+        with_count<1, 2, 4, 8>(P.K / 16, [&](auto ksteps) {         // P.K is 16, 32, 64 or 128 pixels
+            for (int kt = 0; kt < KT; ++kt) {
+                const int s = kt % P.NS;
+                const uint32_t ph = (kt / P.NS) & 1;
+                mbar_wait(&full_bar[s], ph);
+                const uint32_t a_hi = smem_u32(smem + (size_t)s * P.stage_bytes) + a_off;
+                const uint32_t b_hi = smem_u32(smem + (size_t)s * P.stage_bytes) + 2 * P.a_plane;
+                wg_mma3_mn_steps<ksteps>(d, a_hi, a_hi + P.a_plane, b_hi, b_hi + P.b_plane, group, kt != 0);
+                wgmma_commit();
+                wgmma_wait<1>();                               // the previous stage is no longer read
+                if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % P.NS]);
             }
-            wgmma_commit();
-            wgmma_wait<1>();                                   // the previous stage is no longer read
-            if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % P.NS]);
-        }
-        wgmma_wait<0>();
+            wgmma_wait<0>();
+        });
         // fragment element i: output channel 16w + lane/4 + 8*((i>>1)&1), input channels 8*(i>>2) + 2*(lane&3) + {0,1}
 #pragma unroll
         for (int jb = 0; jb < NB; ++jb)

@@ -5,6 +5,7 @@
 
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <type_traits>
 
 namespace effdet {
 
@@ -68,32 +69,94 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// D[64x64] (+)= A[64x16] * B[16x64], bf16 inputs from shared memory, fp32 accumulation in registers.
-// MN = 0: K-major operands, MN = 1: MN-major operands (both A and B).
+// D[64 x 64NB] (+)= A[64x16] * B[16 x 64NB] in ONE wgmma (m64n64k16, m64n128k16 or m64n256k16), bf16 inputs from shared
+// memory, fp32 accumulation in registers.  The accumulator of an m64nNk16 is the NB 64x64 blocks above side by side:
+// registers 32j .. 32j+31 of the instruction are d[j].  MN = 0: K-major operands, MN = 1: MN-major operands (A and B).
+#define EFFDET_WG_D8(a, o) "+f"(a[o]), "+f"(a[o + 1]), "+f"(a[o + 2]), "+f"(a[o + 3]), "+f"(a[o + 4]), "+f"(a[o + 5]), \
+                           "+f"(a[o + 6]), "+f"(a[o + 7])
+#define EFFDET_WG_D32(a) EFFDET_WG_D8(a, 0), EFFDET_WG_D8(a, 8), EFFDET_WG_D8(a, 16), EFFDET_WG_D8(a, 24)
 template <int MN>
-__device__ __forceinline__ void wgmma_64x64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_bf16(float (&d)[1][32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
         "setp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %35;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, %35, %35;\n\t}"
+        : EFFDET_WG_D32(d[0])
         : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(MN)
         : "memory");
 }
-// One K16 step of the split-precision product on NB 64-column blocks: lo*hi + hi*lo + hi*hi (x ~= hi + lo).
-// a_*: this warpgroup's 64-row slice; the B blocks are b_step bytes apart.
-template <int NB, int MN, int NBMAX>
-__device__ __forceinline__ void wg_mma3(float (&d)[NBMAX][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
-                                        uint32_t b_step, uint32_t lbo, uint32_t sbo, uint32_t accumulate) {
+template <int MN>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[2][32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, %67, %67;\n\t}"
+        : EFFDET_WG_D32(d[0]), EFFDET_WG_D32(d[1])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(MN)
+        : "memory");
+}
+template <int MN>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[4][32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+        "}, %128, %129, p, 1, 1, %131, %131;\n\t}"
+        : EFFDET_WG_D32(d[0]), EFFDET_WG_D32(d[1]), EFFDET_WG_D32(d[2]), EFFDET_WG_D32(d[3])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(MN)
+        : "memory");
+}
+#undef EFFDET_WG_D32
+#undef EFFDET_WG_D8
+// One K16 step of the split-precision product over all NB*64 columns: lo*hi + hi*lo + hi*hi (x ~= hi + lo), one
+// full-width wgmma per product, so every accumulator element sums the three products in that order.
+// a_*: this warpgroup's 64-row slice.  The descriptor locates the B operand's 64-column blocks: 8 * sbo bytes apart
+// for K-major operands (64 rows of 128 bytes), lbo bytes apart for MN-major ones.
+template <int NB, int MN>
+__device__ __forceinline__ void wg_mma3(float (&d)[NB][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                        uint32_t lbo, uint32_t sbo, uint32_t accumulate) {
     const uint64_t dah = gmma_desc(a_hi, lbo, sbo), dal = gmma_desc(a_lo, lbo, sbo);
+    const uint64_t dbh = gmma_desc(b_hi, lbo, sbo), dbl = gmma_desc(b_lo, lbo, sbo);
+    wgmma_bf16<MN>(d, dal, dbh, accumulate);
+    wgmma_bf16<MN>(d, dah, dbl, 1);
+    wgmma_bf16<MN>(d, dah, dbh, 1);
+}
+// KS K16 steps of one stage of MN-major operands (the weight gradients: GEMM-K = pixel rows, a K16 step is two 8-row
+// groups, SBO = 1024 bytes apart; 64-channel groups `group` bytes apart), fully unrolled.
+template <int KS, int NB>
+__device__ __forceinline__ void wg_mma3_mn_steps(float (&d)[NB][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                                 uint32_t group, uint32_t accumulate) {
+    wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < NB; ++j) {
-        const uint64_t dbh = gmma_desc(b_hi + j * b_step, lbo, sbo), dbl = gmma_desc(b_lo + j * b_step, lbo, sbo);
-        wgmma_64x64<MN>(d[j], dal, dbh, accumulate);
-        wgmma_64x64<MN>(d[j], dah, dbl, 1);
-        wgmma_64x64<MN>(d[j], dah, dbh, 1);
+    for (int k = 0; k < KS; ++k) {
+        const uint32_t ko = k * 2 * 1024;
+        wg_mma3<NB, 1>(d, a_hi + ko, a_lo + ko, b_hi + ko, b_lo + ko, group, 1024, accumulate | k);
     }
+}
+// Calls f(std::integral_constant<int, n>()) for the one count among KS... that equals n: a warp-uniform branch into one
+// body per count, so that the K16 steps of a stage (a runtime count) are fully unrolled.  ptxas has to see every
+// wgmma of a loop over stages in straight-line code; with a runtime trip count or a branch between the wgmma groups
+// of consecutive stages it fences the accumulator registers (C7519) or serialises the wgmma (C7520).  So the branch
+// goes around the whole loop over stages.
+template <int... KS, class F>
+__device__ __forceinline__ void with_count(const int n, F&& f) {
+    (void)((n == KS && (f(std::integral_constant<int, KS>()), true)) || ...);
 }
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {

@@ -1,7 +1,13 @@
-"""Micro-benchmark of ONE RetinaHead tower layer over the five pyramid levels (the multi-level launches of
-models/_ops.py::RetinaHeadFn) through the C ABI: forward (bias + ReLU), data gradient (ReLU mask) and weight
-gradient.  Every run also prints checksums of the three results so that two builds can be compared.
-usage: python tools/bench_head.py [B] [Cin] [Cout] [size] [iters]"""
+"""Micro-benchmark of the RetinaHead convolutions as models/_ops.py::RetinaHeadPlanesFn runs them: activations and
+gradients as bf16 hi/lo planes, every layer one launch over the five pyramid levels, through the C ABI.  Two shapes:
+a 256->256 tower layer and the 256->720 class conv (9 anchors x 80 classes), each in three directions:
+  fwd    conv_planes_multi, bias + activation (tower: ReLU into planes; class conv: sigmoid into fp32)
+  dgrad  conv_planes_multi on the gradient planes, ReLU mask of the layer input, column sums (bias gradient) -> planes
+  wgrad  wgrad_planes_multi from the input and gradient planes
+Times are CUDA events around `iters` back-to-back launches; TFLOP/s are algorithmic (2 * pixels * 9 * Cin * Cout per
+launch; the tensor cores execute three bf16 products for each).  Every result is also reduced to checksums so that two
+builds can be compared.
+usage: python tools/bench_head.py [B] [size] [iters]"""
 import os
 import sys
 
@@ -11,39 +17,78 @@ import torch                      # noqa: E402
 from models import _native as N   # noqa: E402
 from models import _ops as ops    # noqa: E402
 
-B, Cin, Cout, size, iters = [int(v) for v in (sys.argv[1:6] + ['32', '256', '256', '512', '10'][len(sys.argv) - 1:])]
+B, size, iters = [int(v) for v in (sys.argv[1:4] + ['32', '512', '20'][len(sys.argv) - 1:])]
 dev = torch.device('cuda:0')
 g = torch.Generator(device=dev).manual_seed(0)
-sides = [size >> s for s in (3, 4, 5, 6, 7)]
-w = torch.nn.Parameter(torch.randn(Cout, Cin, 3, 3, device=dev, generator=g) / (Cin * 9) ** 0.5)
-bias = torch.randn(Cout, device=dev, generator=g)
-nbuf = 3                                                        # 3 x ~0.7 GB of activations: every launch misses L2
-xs = [[torch.randn(B, s, s, Cin, device=dev, generator=g) for s in sides] for _ in range(nbuf)]
-dys = [[torch.randn(B, s, s, Cout, device=dev, generator=g) for s in sides] for _ in range(nbuf)]
-wf, wd = ops.pack_conv(w)
-tf, td = ops.pack_conv_tc(w)
-tc = ops.tc_enabled()
-dw = torch.zeros_like(w)
-db = torch.zeros(Cout, device=dev)
+sides = [size >> s for s in (3, 4, 5, 6, 7)]                  # P3..P7
+geo = [(B, s, s) for s in sides]
+px = B * sum(s * s for s in sides)
+NBUF = 3                                                       # rotating operand sets: every launch misses L2
 
 
-def fwd(i):
-    return ops.conv2d_multi(xs[i % nbuf], wf, Cout, 3, bias=bias, act=N.ACT_RELU, w_tc=tf if tc else None)
+def planes_of(C, relu=False):
+    """random NHWC fp32 maps of every level -> bf16 hi/lo planes (ReLU'd: a tower activation, the dgrad mask)"""
+    out = []
+    for (b, h, w) in geo:
+        x = torch.randn(b, h, w, C, device=dev, generator=g)
+        if relu:
+            x = x.clamp_min_(0.0)
+        p = ops._planes(b, h, w, C, x)
+        ops.to_planes(N.f32(x), h * w * C, p, b, h * w, C, x)
+        out.append(p)
+    return out
 
 
-def dgrad(i):
-    return ops.conv2d_multi(dys[i % nbuf], wd, Cin, 3, w_tc=td if tc else None, masks=xs[i % nbuf])
+def planes_sum(ps):
+    return [float(sum((p[0].double() + p[1].double()).sum() for p in ps)),
+            float(sum((p[0].double() + p[1].double()).abs().sum() for p in ps))]
 
 
-def wgrad(i):
-    lv = [dict(x_ptr=N.f32(x), x_bs=x.shape[1] * x.shape[2] * Cin, dy_ptr=N.f32(d), dy_bs=d.shape[1] * d.shape[2] * Cout,
-               B=B, H=x.shape[1], W=x.shape[2]) for x, d in zip(xs[i % nbuf], dys[i % nbuf])]
-    ops.conv_wgrad_multi(xs[0][0], lv, dw, db, Cin, Cout, 3, tc=tc)
-    return [dw]
+def shape(Cin, Cout, act):
+    w = torch.randn(Cout, Cin, 3, 3, device=dev, generator=g) / (Cin * 9) ** 0.5
+    bias = torch.randn(Cout, device=dev, generator=g)
+    tf, td = ops.pack_conv_tc(w)
+    xs = [planes_of(Cin, relu=True) for _ in range(NBUF)]     # layer inputs (post-ReLU tower activations)
+    dys = [planes_of(Cout) for _ in range(NBUF)]              # gradients w.r.t. the layer outputs
+    if act == N.ACT_RELU:
+        ys = [ops._planes(b, h, wd, Cout, w) for (b, h, wd) in geo]
+        fwd_lv = [dict(y_planes=ys[l]) for l in range(len(geo))]
+    else:
+        ys = [torch.empty(b, h, wd, Cout, device=dev) for (b, h, wd) in geo]
+        fwd_lv = [dict(y_ptr=N.f32(ys[l]), y_bs=geo[l][1] * geo[l][2] * Cout) for l in range(len(geo))]
+    dxs = [ops._planes(b, h, wd, Cin, w) for (b, h, wd) in geo]
+    colsum = torch.zeros(Cin, device=dev)
+    dw = torch.zeros_like(w)
+
+    def fwd(i):
+        ops.conv_planes_multi(w, [dict(x=xs[i % NBUF][l], B=b, H=h, W=wd, **fwd_lv[l]) for l, (b, h, wd) in enumerate(geo)],
+                              tf, Cin, Cout, 3, bias=bias, act=act)
+
+    def dgrad(i):
+        ops.conv_planes_multi(w, [dict(x=dys[i % NBUF][l], y_planes=dxs[l], mask=xs[i % NBUF][l], B=b, H=h, W=wd)
+                                  for l, (b, h, wd) in enumerate(geo)], td, Cout, Cin, 3, colsum=colsum)
+
+    def wgrad(i):
+        ops.wgrad_planes_multi(w, [dict(x=xs[i % NBUF][l], dy=dys[i % NBUF][l], B=b, H=h, W=wd)
+                                   for l, (b, h, wd) in enumerate(geo)], dw, Cin, Cout, 3)
+
+    def checksum(name):
+        colsum.zero_()
+        dw.zero_()
+        {'fwd': fwd, 'dgrad': dgrad, 'wgrad': wgrad}[name](0)
+        if name == 'fwd':
+            if act == N.ACT_RELU:
+                return planes_sum(ys)
+            return [float(sum(y.double().sum() for y in ys)), float(sum(y.double().abs().sum() for y in ys))]
+        if name == 'dgrad':
+            return planes_sum(dxs) + [float(colsum.double().sum())]
+        return [float(dw.double().sum()), float(dw.double().abs().sum())]
+
+    return dict(fwd=fwd, dgrad=dgrad, wgrad=wgrad), checksum
 
 
 def timed(fn):
-    for i in range(2):
+    for i in range(NBUF):
         fn(i)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -55,16 +100,14 @@ def timed(fn):
     return e0.elapsed_time(e1) / iters
 
 
-px = B * sum(s * s for s in sides)
-flops = 2.0 * px * 9 * Cin * Cout
-print('levels', sides, 'B', B, '%d->%d' % (Cin, Cout), 'precision', ops.PRECISION)
-for name, fn in (('fwd', fwd), ('dgrad', dgrad), ('wgrad', wgrad)):
-    if name == 'wgrad':
-        dw.zero_(); db.zero_()
-        out = fn(0)
-        chk = [float(dw.double().sum()), float(dw.double().abs().sum()), float(db.double().sum())]
-    else:
-        out = fn(0)
-        chk = [float(sum(o.double().sum() for o in out)), float(sum(o.double().abs().sum() for o in out))]
-    ms = timed(fn)
-    print('%-6s %.3f ms  %.1f TFLOP/s algorithmic   checksum %s' % (name, ms, flops / ms / 1e9, ['%.6e' % c for c in chk]))
+print('levels', sides, 'B', B, 'pixels', px, 'iters', iters, 'device', torch.cuda.get_device_name(dev))
+for Cin, Cout, act in ((256, 256, N.ACT_RELU), (256, 720, N.ACT_SIGMOID)):
+    fns, checksum = shape(Cin, Cout, act)
+    flops = 2.0 * px * 9 * Cin * Cout
+    for name in ('fwd', 'dgrad', 'wgrad'):
+        chk = checksum(name)
+        ms = timed(fns[name])
+        print('%d->%d %-6s %8.3f ms  %6.1f TFLOP/s algorithmic   checksum %s'
+              % (Cin, Cout, name, ms, flops / ms / 1e9, ['%.9e' % c for c in chk]), flush=True)
+    del fns, checksum
+    torch.cuda.empty_cache()
