@@ -1,8 +1,12 @@
 // Dense 3x3 / 1x1 convolution whose activations live in HBM as bf16 hi/lo planes (x ~= hi + lo, the tensor-core operand
 // format) -- the RetinaHead towers end to end (models/retinahead.py:67-132; 95 % of the model's FLOPs).
 //
-// Round 1 kept fp32 activations: every conv re-split its input on the fly with eight gather warps (LDG + cvt + st.shared)
-// and every weight gradient needed a separate split pass over both operands (~190 launches, ~3 ms per step).  With the
+//   conv_planes_kernel  the convolution below
+//   to_planes_kernel    fp32 -> planes, for the head's first input, its output gradients and the operands of the TMA-fed
+//                       weight gradient (conv_tc.cu) that are not planes yet
+//
+// Kept as fp32, every conv would re-split its input on the fly with eight gather warps (LDG + cvt + st.shared) and every
+// weight gradient would need a separate split pass over both operands.  With the
 // planes format the im2col gather IS a TMA load: a 5-D tensor map (channel, x, y, image, plane) with a pixel box of
 // Wb x Hb x Bb pixels delivers, for one tap, 64 channels of 16..64 pixels as consecutive 128-byte rows in the canonical
 // K-major SWIZZLE_128B layout; the tap shift is a coordinate offset and the hardware's out-of-bounds zero fill is the
@@ -325,6 +329,26 @@ __global__ void __launch_bounds__(256) to_planes_kernel(const float* __restrict_
     }
 }
 
+int to_planes_launch(const float* x, long long x_bstride, const float* prob, long long p_bstride, void* out, float* colsum,
+                     int B, int HW, int C, int pitch, cudaStream_t st) {
+    const int cv8 = pitch / 8;
+    const int cvb = cv8 < 256 ? cv8 : 256;
+    const int rows = 256 / cvb;
+    const long long nrows = (long long)B * HW;
+    const int ychunks = cdiv(cv8, cvb);
+    long long rpb;
+    if (colsum) {           // ~4 waves of blocks, at least 8 row iterations each: few atomics per column
+        rpb = (nrows + num_sms() * 4 - 1) / (num_sms() * 4);
+        if (rpb < (long long)rows * 8) rpb = (long long)rows * 8;
+    } else {                // nothing to amortise: up to 16 blocks per SM, down to one row iteration each
+        rpb = (nrows * ychunks + num_sms() * 16 - 1) / (num_sms() * 16);
+        if (rpb < rows) rpb = rows;
+    }
+    dim3 grid(cdiv(nrows, rpb), ychunks);
+    to_planes_kernel<<<grid, 256, 0, st>>>(x, x_bstride, prob, p_bstride, (__nv_bfloat16*)out, colsum, B, HW, C, pitch, (int)rpb);
+    return launch_status("to_planes_kernel");
+}
+
 }  // namespace effdet
 
 using namespace effdet;
@@ -335,17 +359,7 @@ extern "C" int effdet_to_planes(const float* x, int64_t x_bstride, const float* 
     EFFDET_REQUIRE(aligned16(x) && aligned16(prob) && aligned16(planes) && x_bstride % 4 == 0 && p_bstride % 4 == 0,
                    "to_planes: alignment");
     EFFDET_DEVICE(device);
-    const int pitch = (C + 7) / 8 * 8;
-    const int cv8 = pitch / 8;
-    const int cvb = cv8 < 256 ? cv8 : 256;
-    const int rows = 256 / cvb;
-    const long long nrows = (long long)B * HW;
-    long long rpb = (nrows + num_sms() * 4 - 1) / (num_sms() * 4);
-    if (rpb < (long long)rows * 8) rpb = (long long)rows * 8;
-    dim3 grid(cdiv(nrows, rpb), cdiv(cv8, cvb));
-    to_planes_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, x_bstride, prob, p_bstride, (__nv_bfloat16*)planes, colsum, B, HW, C,
-                                                            pitch, (int)rpb);
-    return launch_status("to_planes_kernel");
+    return to_planes_launch(x, x_bstride, prob, p_bstride, planes, colsum, B, HW, C, (C + 7) / 8 * 8, (cudaStream_t)stream);
 }
 
 extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, int nlevels, int device, effdet_stream_t stream) {
@@ -395,16 +409,8 @@ extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, i
     // 128 x 128 tiles at most: the accumulator lives in the consumer warpgroups' registers (64 per thread)
     const int BN = a0->Cout <= 64 ? 64 : 128;
     CUtensorMap wmap;
-    {
-        const cuuint64_t gdim[3] = {(cuuint64_t)taps * kpad, (cuuint64_t)a0->Cout, 2};
-        const cuuint64_t gstr[2] = {(cuuint64_t)taps * kpad * 2, (cuuint64_t)a0->Cout * taps * kpad * 2};
-        const cuuint32_t box[3] = {64, (cuuint32_t)BN, 1};
-        const cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(a0->w_tc), gdim, gstr, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return fail(EFFDET_ERR_LAUNCH, "conv_planes_multi: tensor map of the weights failed (%d)", (int)r);
-    }
+    const int s = kmajor_planes_map(enc, &wmap, a0->w_tc, a0->Cout, taps * kpad, BN);
+    if (s) return s;
     P.nlevels = nlevels;
     P.ntn = cdiv(a0->Cout, BN);
     P.total_tiles = tiles * P.ntn;
@@ -414,15 +420,7 @@ extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, i
     P.bias = a0->bias;
     P.colsum = a0->colsum;
     const int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
-#define EFFDET_PL_LAUNCH(BN_)                                                                                              \
-    do {                                                                                                                  \
-        cudaError_t e = cudaFuncSetAttribute(conv_planes_kernel<BN_>, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
-                                             PlCfg<BN_>::kSmem);                                                          \
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "conv_planes_multi: smem opt-in: %s", cudaGetErrorString(e)); \
-        conv_planes_kernel<BN_><<<grid, kPlThreads, PlCfg<BN_>::kSmem, (cudaStream_t)stream>>>(maps, wmap, P);             \
-    } while (0)
-    if (BN == 64) EFFDET_PL_LAUNCH(64);
-    else EFFDET_PL_LAUNCH(128);
-#undef EFFDET_PL_LAUNCH
-    return launch_status("conv_planes_kernel");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (BN == 64) return launch_smem("conv_planes_kernel", conv_planes_kernel<64>, grid, kPlThreads, PlCfg<64>::kSmem, st, maps, wmap, P);
+    return launch_smem("conv_planes_kernel", conv_planes_kernel<128>, grid, kPlThreads, PlCfg<128>::kSmem, st, maps, wmap, P);
 }

@@ -12,7 +12,7 @@ namespace effdet {
 
 // tensor-core path (conv_tc.cu)
 bool conv_tc_eligible(const effdet_conv_args* a);
-int conv_tc_launch(const effdet_conv_args* a, cudaStream_t st);
+int conv_tc_launch(const effdet_conv_args* levels, int nlevels, cudaStream_t st);
 bool wgrad_tc_eligible(const effdet_wgrad_args* a);
 bool pw_wgrad_eligible(const effdet_wgrad_args* a);
 int pw_wgrad_launch(const effdet_wgrad_args* a, cudaStream_t st);
@@ -393,7 +393,7 @@ extern "C" int effdet_conv2d(const effdet_conv_args* a, int device, effdet_strea
     EFFDET_REQUIRE(Mll < (1ll << 31), "conv2d: B*H*W too large");
     const int M = (int)Mll, HW = a->H * a->W;
     if (pw_gemm_eligible(a)) return pw_gemm_launch(a, (cudaStream_t)stream);
-    if (conv_tc_eligible(a)) return conv_tc_launch(a, (cudaStream_t)stream);
+    if (conv_tc_eligible(a)) return conv_tc_launch(a, 1, (cudaStream_t)stream);
     // pick the N tile that wastes the fewest padded columns (ties -> wider tile)
     int best = 128;
     long long best_pad = (long long)cdiv(a->Cout, 128) * 128;
@@ -460,8 +460,8 @@ extern "C" int effdet_conv2d_wgrad(const effdet_wgrad_args* a, int device, effde
     } else if (wgrad_tc_eligible(a)) {
         s = wgrad_tc_launch(a, st, &dbias_done);
     } else if (a->dy_planes || a->x_planes) {
-        return fail(EFFDET_ERR_UNSUPPORTED, "wgrad: dy_planes given but the TMA-fed tensor-core kernel cannot take this shape "
-                                            "(check effdet_wgrad_tc_geometry_ok first)");
+        return fail(EFFDET_ERR_UNSUPPORTED, "wgrad: dy_planes given but the TMA-fed tensor-core kernel cannot take this shape or "
+                                            "input prologue (check effdet_wgrad_tc_geometry_ok first)");
     } else {
     int BC, BN;
     if (a->Cin <= 32) { BC = 32; BN = 128; }

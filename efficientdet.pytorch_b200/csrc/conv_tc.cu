@@ -1,6 +1,11 @@
-// Tensor-core (wgmma) implicit-GEMM convolution for the dense 3x3 (and 1x1) layers of head and
-// neck: forward, data gradient (same kernel on the rotated/transposed weight pack) and weight
+// Tensor-core (wgmma) implicit-GEMM convolution for the dense 3x3 layers of head and neck:
+// forward, data gradient (same kernel on the rotated/transposed weight pack) and weight
 // gradient.  95 % of the model's FLOPs live here (SURVEY.md section 0 fact 3).
+//   conv_tc_kernel          forward / data gradient, fp32 activations gathered and split in the kernel,
+//                           every pyramid level that shares the weights in one launch
+//   wgrad_tc2_multi_kernel  weight gradient fed by TMA from bf16 hi/lo planes (to_planes_kernel splits the
+//                           operands that are not planes yet), every level in one launch
+//   wgrad_tc_kernel         weight gradient that gathers and splits fp32 operands itself: maps with no pixel box
 //
 // Precision: operands stay fp32 in HBM (module API parity) and are split on the fly into
 // bf16 hi + bf16 lo (x = hi + lo to 16 mantissa bits); every product is evaluated as
@@ -20,14 +25,10 @@
 // MN-major operands), split-K over pixel ranges with fp32 atomics into the OIHW gradient.
 #include "tc_ptx.cuh"
 
-#include <stdlib.h>
-
 namespace effdet {
 
-constexpr int kTcThreads = 288;        // two MMA / epilogue warpgroups + one TMA warp
-constexpr int kTcProducers = 256;      // gathering weight-gradient kernel: two gather / MMA / epilogue warpgroups
-constexpr int kFwdThreads = 288;       // forward/dgrad kernel: two gather / MMA / epilogue warpgroups + TMA
-constexpr int kFwdProducers = 256;
+constexpr int kTcThreads = 288;        // two gather / MMA / epilogue warpgroups + one TMA warp
+constexpr int kTcProducers = 256;      // the two warpgroups (all of the gathering weight-gradient kernel)
 constexpr int kTileM = 128;     // pixels per CTA (fwd/dgrad) or output channels per CTA (wgrad)
 constexpr int kTileK = 64;      // bf16 elements per 128-byte swizzled row
 
@@ -39,30 +40,42 @@ struct FwdSmem {
     static constexpr int kA = kTileM * 128;   // bytes of one bf16 plane of the A tile
     static constexpr int kB = BN * 128;       // bytes of one bf16 plane of the B tile
     static constexpr int kStage = 2 * kA + 2 * kB;
-    static constexpr int kChan = 3 * BN * 4;  // bias | scale | shift of this CTA's output channels
+    static constexpr int kChan = BN * 4;      // bias of this CTA's output channels
     static constexpr int kBytes = STAGES * kStage + 1024 /*alignment slack*/ + 256 /*barriers*/ + kChan;
 };
 
-// MB = true adds the MBConv-only pieces (BN+swish / SE gate on the input, raw-output save, BN affine, drop-connect scale)
-template <int BN, int STAGES, bool MB>
-__device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effdet_conv_args& p, const int M, const int HW,
-                                             const int kblocks, const int m0, const int n0) {
+// Several pyramid levels that share one weight tensor (RetinaHead runs the same convs on P3..P7,
+// models/retinahead.py:131-132) in ONE launch: the M tiles of all levels are concatenated so the small
+// levels (a handful of CTAs each) ride along with the large ones instead of paying their own latency-bound launch.
+constexpr int kMaxLevels = 8;
+struct ConvMultiArgs {
+    effdet_conv_args lv[kMaxLevels];
+    int tile_begin[kMaxLevels + 1];
+    int nlevels;
+};
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kTcThreads, 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ ConvMultiArgs ma, const int kblocks) {
     using S = FwdSmem<BN, STAGES>;
+    const int tile = blockIdx.x;
+    int l = 0;
+    while (l + 1 < ma.nlevels && tile >= ma.tile_begin[l + 1]) ++l;
+    const effdet_conv_args& p = ma.lv[l];
+    const int M = p.B * p.H * p.W, HW = p.H * p.W;
+    const int m0 = (tile - ma.tile_begin[l]) * kTileM, n0 = blockIdx.y * BN;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1024-byte aligned AND still a shared-space pointer (LDS/STS, not generic LD/ST)
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::kStage);
     uint64_t* empty_bar = full_bar + STAGES;
-    float* chan = reinterpret_cast<float*>(smem + STAGES * S::kStage + 256);   // [3][BN]
+    float* chan = reinterpret_cast<float*>(smem + STAGES * S::kStage + 256);   // [BN]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int taps = p.ksize * p.ksize, pad = p.ksize / 2;
     const int KT = taps * kblocks;
-    for (int i = threadIdx.x; i < BN; i += kFwdThreads) {
+    for (int i = threadIdx.x; i < BN; i += kTcThreads) {
         const int n = n0 + i;
-        const bool ok = n < p.Cout;
-        chan[i] = (ok && p.bias) ? __ldg(p.bias + n) : 0.f;
-        chan[BN + i] = (MB && ok && p.scale) ? __ldg(p.scale + n) : 1.f;
-        chan[2 * BN + i] = (MB && ok && p.shift) ? __ldg(p.shift + n) : 0.f;
+        chan[i] = (n < p.Cout && p.bias) ? __ldg(p.bias + n) : 0.f;
     }
 
     if (threadIdx.x == 0) {
@@ -116,42 +129,14 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effd
                 }
             }
         };
-        // input prologue of the MBConv project conv: eval-BN + swish of the raw depthwise output, then the
-        // squeeze-excite gate.  Zero-filled elements (rows beyond M, channels beyond Cin) must stay zero.
-        auto prologue = [&](int kt, float4 (&v)[8]) {
-            const int tap = kt / kblocks;
-            const int c = (kt - tap * kblocks) * kTileK + j * 8;
-            if (c >= p.Cin) return;
-            const bool hi_ok = c + 4 < p.Cin;
-            float4 s0 = make_float4(1.f, 1.f, 1.f, 1.f), s1 = s0, h0 = f4zero(), h1 = f4zero();
-            if (p.in_scale) {
-                s0 = ldg4(p.in_scale + c); h0 = ldg4(p.in_shift + c);
-                if (hi_ok) { s1 = ldg4(p.in_scale + c + 4); h1 = ldg4(p.in_shift + c + 4); }
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                if (oyx[i] < 0) continue;
-                if (p.in_scale) {
-                    const float4 u0 = f4fma(v[2 * i], s0, h0), u1 = f4fma(v[2 * i + 1], s1, h1);
-                    v[2 * i] = make_float4(swishf_(u0.x), swishf_(u0.y), swishf_(u0.z), swishf_(u0.w));
-                    v[2 * i + 1] = hi_ok ? make_float4(swishf_(u1.x), swishf_(u1.y), swishf_(u1.z), swishf_(u1.w)) : f4zero();
-                }
-                if (p.a_scale) {                               // squeeze-excite gate on the input (per image, channel)
-                    const float* gp = p.a_scale + (base[i] / p.x_bstride) * p.Cin + c;
-                    v[2 * i] = f4mul(v[2 * i], ldg4(gp));
-                    if (hi_ok) v[2 * i + 1] = f4mul(v[2 * i + 1], ldg4(gp + 4));
-                }
-            }
-        };
         float d[NB][32];
         for (int kt = 0; kt < KT; ++kt) {
             const int s = kt % STAGES;
             const uint32_t ph = (kt / STAGES) & 1;
             float4 v[8];
             load_stage(kt, v);                   // in flight while the previous stage's wgmma run
-            if (MB && (p.in_scale || p.a_scale)) prologue(kt, v);
             wgmma_wait<STAGES - 1>();            // this warpgroup no longer reads stage s ...
-            named_bar_sync(1, kFwdProducers);    // ... nor does the other one
+            named_bar_sync(1, kTcProducers);     // ... nor does the other one
             if (t == 0 && kt >= STAGES) mbar_arrive(&empty_bar[s]);
             uint8_t* a_hi = smem + s * S::kStage;
             uint8_t* a_lo = a_hi + S::kA;
@@ -165,7 +150,7 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effd
                 *reinterpret_cast<uint4*>(a_lo + off) = lo;
             }
             fence_proxy_async();
-            named_bar_sync(1, kFwdProducers);    // the A tile is complete
+            named_bar_sync(1, kTcProducers);     // the A tile is complete
             mbar_wait(&full_bar[s], ph);         // the weight tile landed
             const uint32_t sa = smem_u32(a_hi) + g * 64 * 128;
             const uint32_t sb = smem_u32(a_hi) + 2 * S::kA;
@@ -176,7 +161,7 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effd
             wgmma_commit();
         }
         wgmma_wait<0>();
-        named_bar_sync(1, kFwdProducers);        // every stage is drained: stage 0 becomes the epilogue's staging buffer
+        named_bar_sync(1, kTcProducers);         // every stage is drained: stage 0 becomes the epilogue's staging buffer
         // ---------------- epilogue ------------------------------------------------------------------------------------
         float* rows_buf = reinterpret_cast<float*>(smem);
         const int quarter = 2 * g + (warp & 1), half = (warp >> 1) & 1;   // 32-row group, 32-column chunk parity
@@ -188,7 +173,6 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effd
             b = m / HW;
             pix = m - b * HW;
         }
-        const float rs = (MB && row_ok && p.row_scale) ? __ldg(p.row_scale + b) : 1.f;
         const int ncols = min(BN, p.Cout - n0);
         const int nchunks = (ncols + 31) >> 5;
         const long long ybase = (long long)b * p.y_bstride + pix * p.Cout;
@@ -207,8 +191,6 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effd
                 if (n >= p.Cout) break;
                 float4 v = make_float4(acc[q * 4], acc[q * 4 + 1], acc[q * 4 + 2], acc[q * 4 + 3]);
                 v = f4add(v, *reinterpret_cast<const float4*>(chan + nl));
-                if (MB && p.z) st4(p.z + ybase + n, v);
-                if (MB) v = f4fma(v, *reinterpret_cast<const float4*>(chan + BN + nl), *reinterpret_cast<const float4*>(chan + 2 * BN + nl));
                 if (p.act == EFFDET_ACT_RELU) {
                     v = make_float4(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f), fmaxf(v.z, 0.f), fmaxf(v.w, 0.f));
                 } else if (p.act == EFFDET_ACT_SIGMOID) {
@@ -216,7 +198,6 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effd
                 } else if (p.act == EFFDET_ACT_SWISH) {
                     v = make_float4(swishf_(v.x), swishf_(v.y), swishf_(v.z), swishf_(v.w));
                 }
-                if (MB && p.row_scale) v = f4scale(v, rs);
                 if (p.residual) v = f4add(v, ldg4(p.residual + rbase + n));
                 if (p.mask_src) {
                     const float4 mv = ldg4(p.mask_src + mbase + n);
@@ -239,34 +220,6 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& wmap, const effd
             }
         }
     }
-}
-
-template <int BN, int STAGES, bool MB>
-__global__ void __launch_bounds__(kFwdThreads, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ effdet_conv_args p, const int M, const int HW,
-               const int kblocks) {
-    conv_tc_body<BN, STAGES, MB>(wmap, p, M, HW, kblocks, blockIdx.x * kTileM, blockIdx.y * BN);
-}
-
-// Several pyramid levels that share one weight tensor (RetinaHead runs the same convs on P3..P7,
-// models/retinahead.py:131-132) in ONE launch: the M tiles of all levels are concatenated so the small
-// levels (a handful of CTAs each) ride along with the large ones instead of paying their own latency-bound launch.
-constexpr int kMaxLevels = 8;
-struct ConvMultiArgs {
-    effdet_conv_args lv[kMaxLevels];
-    int tile_begin[kMaxLevels + 1];
-    int nlevels;
-};
-
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(kFwdThreads, 1)
-conv_tc_multi_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ ConvMultiArgs ma, const int kblocks) {
-    const int tile = blockIdx.x;
-    int l = 0;
-    while (l + 1 < ma.nlevels && tile >= ma.tile_begin[l + 1]) ++l;
-    const effdet_conv_args& p = ma.lv[l];
-    conv_tc_body<BN, STAGES, false>(wmap, p, p.B * p.H * p.W, p.H * p.W, kblocks, (tile - ma.tile_begin[l]) * kTileM,
-                                    blockIdx.y * BN);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -377,114 +330,17 @@ wgrad_tc_kernel(const effdet_wgrad_args p, const int M, const int HW, const int 
 }
 
 // ---------------------------------------------------------------------------------------------
-// weight-gradient kernel, TMA-fed: the operands were pre-split into bf16 hi/lo planes
-// [2][B][H][W][Cpad] by split_planes_kernel, so the gather warps disappear: one thread issues
-// 5-D tensor-map loads (channel group, x, y, image, plane) whose out-of-bounds zero fill IS the
-// convolution's zero padding (the tap shift is just a coordinate offset); two consumer warpgroups
-// (64 output channels each) issue the wgmma and add their accumulators to the OIHW gradient with
-// atomics.  A stage covers a box of
+// weight-gradient kernel, TMA-fed: the operands are bf16 hi/lo planes [2][B][H][W][Cpad]
+// (split by to_planes_kernel, or written in that form by their producer), so the gather warps
+// disappear: one thread issues 5-D tensor-map loads (channel group, x, y, image, plane) whose
+// out-of-bounds zero fill IS the convolution's zero padding (the tap shift is just a coordinate
+// offset); two consumer warpgroups (64 output channels each) issue the wgmma and add their
+// accumulators to the OIHW gradient with atomics.  A stage covers a box of
 // kstage = Wb*Hb*Bb pixels (<= 64, multiple of 16).
+// The pixel chunks of several pyramid levels (same weights, e.g. the five RetinaHead levels) form
+// one long GEMM-K dimension, so one launch covers them all; each chunk looks up its level's tensor
+// maps and pixel-box geometry.
 // ---------------------------------------------------------------------------------------------
-EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    }
-    return fn;
-}
-
-int conv_tc_kpad(int k) { return (k + kTileK - 1) / kTileK * kTileK; }
-
-template <int BC, int STAGES>
-__global__ void __launch_bounds__(kTcThreads, 1)
-wgrad_tc2_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x, const effdet_wgrad_args p,
-                 const WgGeom g, const int chunks_per_split, const int ctiles) {
-    using S = WgSmem<BC, STAGES>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1024-byte aligned AND still a shared-space pointer (LDS/STS, not generic LD/ST)
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::kStage);
-    uint64_t* empty_bar = full_bar + STAGES;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int ct = blockIdx.x % ctiles, nt = blockIdx.x / ctiles;
-    const int c0 = ct * BC, n0 = nt * kTileM;
-    const int tap = blockIdx.y;
-    const int pad = p.ksize / 2;
-    const int dy = tap / p.ksize - pad, dx = tap % p.ksize - pad;
-    const int nchunks = g.nbx * g.nby * g.nbb;
-    const int ch_begin = blockIdx.z * chunks_per_split;
-    const int ch_end = min(nchunks, ch_begin + chunks_per_split);
-    const int KT = ch_end - ch_begin;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 8);     // one arrival per consumer warp
-        }
-        fence_barrier_init();
-    }
-    __syncthreads();
-    constexpr int GROUP = kTileK * 128;            // smem slot of one 64-channel group of one plane
-
-    if (warp == 8) {
-        if (lane == 0) {
-            const uint32_t bytes = (uint32_t)(2 * (kTileM / 64 + BC / 64) * g.kstage * 128);
-            for (int kt = 0; kt < KT; ++kt) {
-                const int s = kt % STAGES;
-                const uint32_t ph = (kt / STAGES) & 1;
-                int ch = ch_begin + kt;
-                const int bx = ch % g.nbx;
-                ch /= g.nbx;
-                const int by = ch % g.nby;
-                const int bb = ch / g.nby;
-                const int x0 = bx * g.Wb, y0 = by * g.Hb, b0 = bb * g.Bb;
-                mbar_wait(&empty_bar[s], ph ^ 1);
-                mbar_arrive_expect_tx(&full_bar[s], bytes);
-                uint8_t* a_hi = smem + s * S::kStage;
-                uint8_t* b_hi = a_hi + 2 * S::kA;
-#pragma unroll
-                for (int pl = 0; pl < 2; ++pl) {
-#pragma unroll
-                    for (int q = 0; q < kTileM / 64; ++q)
-                        tma_load_5d(a_hi + pl * S::kA + q * GROUP, &map_dy, &full_bar[s], n0 + q * 64, x0, y0, b0, pl);
-#pragma unroll
-                    for (int q = 0; q < BC / 64; ++q)
-                        tma_load_5d(b_hi + pl * S::kB + q * GROUP, &map_x, &full_bar[s], c0 + q * 64, x0 + dx, y0 + dy, b0, pl);
-                }
-            }
-        }
-    } else {
-        // two consumer warpgroups: wgmma on output channels n0 + 64 * wg .. + 63, then atomics into OIHW
-        constexpr int NB = BC / 64;
-        const int wg = warp >> 2;
-        float d[NB][32];
-        with_count<1, 2, 3, 4>(g.kstage / 16, [&](auto ksteps) {
-            for (int kt = 0; kt < KT; ++kt) {
-                const int s = kt % STAGES;
-                const uint32_t ph = (kt / STAGES) & 1;
-                mbar_wait(&full_bar[s], ph);
-                const uint32_t sa = smem_u32(smem + s * S::kStage) + wg * GROUP;
-                const uint32_t sb = smem_u32(smem + s * S::kStage) + 2 * S::kA;
-                wg_mma3_mn_steps<ksteps>(d, sa, sa + S::kA, sb, sb + S::kB, GROUP, kt != 0);
-                wgmma_commit();
-                wgmma_wait<1>();                   // the previous stage is no longer read
-                if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % STAGES]);
-            }
-        });
-        wgmma_wait<0>();
-        wg_atomic_dw<NB>(d, p.dw, n0 + 64 * wg, c0, p.Cout, p.Cin, p.ksize * p.ksize, tap);
-    }
-}
-
-// Multi-level variant: the pixel chunks of several pyramid levels (same weights, e.g. the five RetinaHead levels)
-// form one long GEMM-K dimension, so one launch covers them all; each chunk looks up its level's tensor maps and
-// pixel-box geometry.
 constexpr int kWgMaxLevels = 8;
 struct WgMaps {
     CUtensorMap dy[kWgMaxLevels];
@@ -586,117 +442,6 @@ wgrad_tc2_multi_kernel(const __grid_constant__ WgMaps maps, const __grid_constan
     }
 }
 
-// fp32 [B][HW][C] (image stride bstride) -> bf16 planes [2][B*HW][Cpad], zero padded channels
-__global__ void __launch_bounds__(256) split_planes_kernel(const float* __restrict__ x, long long bstride, const float* __restrict__ a_scale,
-                                                           __nv_bfloat16* __restrict__ out, int B, int HW, int C, int Cpad,
-                                                           const float* __restrict__ in_scale = nullptr,
-                                                           const float* __restrict__ in_shift = nullptr) {
-    const int cv = Cpad / 8;
-    const long long total = (long long)B * HW * cv;
-    const long long plane = (long long)B * HW * Cpad;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int j = (int)(i % cv);
-        const long long row = i / cv;
-        const int b = (int)(row / HW);
-        const long long pix = row - (long long)b * HW;
-        const int c = j * 8;
-        float4 v0 = f4zero(), v1 = f4zero();
-        if (c < C) {
-            const float* q = x + (long long)b * bstride + pix * C + c;
-            v0 = ldg4(q);
-            if (c + 4 < C) v1 = ldg4(q + 4);
-            if (in_scale) {                        // operand = swish(bn(x)) of a raw conv output (pre-activation only in HBM)
-                const float4 u0 = f4fma(v0, ldg4(in_scale + c), ldg4(in_shift + c));
-                v0 = make_float4(swishf_(u0.x), swishf_(u0.y), swishf_(u0.z), swishf_(u0.w));
-                if (c + 4 < C) {
-                    const float4 u1 = f4fma(v1, ldg4(in_scale + c + 4), ldg4(in_shift + c + 4));
-                    v1 = make_float4(swishf_(u1.x), swishf_(u1.y), swishf_(u1.z), swishf_(u1.w));
-                }
-            }
-            if (a_scale) {
-                v0 = f4mul(v0, ldg4(a_scale + (long long)b * C + c));
-                if (c + 4 < C) v1 = f4mul(v1, ldg4(a_scale + (long long)b * C + c + 4));
-            }
-        }
-        uint4 hi, lo;
-        split8(v0, v1, hi, lo);
-        *reinterpret_cast<uint4*>(out + row * Cpad + c) = hi;
-        *reinterpret_cast<uint4*>(out + plane + row * Cpad + c) = lo;
-    }
-}
-
-// split + per-channel column sums in one pass: the weight gradient's dy operand is split into planes AND reduced
-// into the bias gradient (dbias[n] += sum over pixels) while it streams by, so no second read of dy.
-__global__ void __launch_bounds__(256) split_planes_colsum_kernel(const float* __restrict__ x, long long bstride,
-                                                                  __nv_bfloat16* __restrict__ out, float* __restrict__ colsum,
-                                                                  int B, int HW, int C, int Cpad, int rows_per_block) {
-    __shared__ float red[256 * 8];
-    const int cv8 = Cpad / 8;
-    const int cvb = cv8 < 256 ? cv8 : 256;
-    const int rows = 256 / cvb;
-    const int tr = threadIdx.x / cvb, tc = threadIdx.x - tr * cvb;
-    const int j = blockIdx.y * cvb + tc;
-    const bool active = tr < rows && j < cv8;
-    const long long nrows = (long long)B * HW;
-    const long long plane = nrows * Cpad;
-    float s[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s[i] = 0.f;
-    if (active) {
-        const int c = j * 8;
-        const long long r_begin = (long long)blockIdx.x * rows_per_block;
-        const long long r_end = min(nrows, r_begin + rows_per_block);
-        for (long long row = r_begin + tr; row < r_end; row += rows) {
-            const int b = (int)(row / HW);
-            const long long pix = row - (long long)b * HW;
-            float4 v0 = f4zero(), v1 = f4zero();
-            if (c < C) {
-                const float* q = x + (long long)b * bstride + pix * C + c;
-                v0 = ldg4(q);
-                if (c + 4 < C) v1 = ldg4(q + 4);
-            }
-            uint4 hi, lo;
-            split8(v0, v1, hi, lo);
-            *reinterpret_cast<uint4*>(out + row * Cpad + c) = hi;
-            *reinterpret_cast<uint4*>(out + plane + row * Cpad + c) = lo;
-            s[0] += v0.x; s[1] += v0.y; s[2] += v0.z; s[3] += v0.w;
-            s[4] += v1.x; s[5] += v1.y; s[6] += v1.z; s[7] += v1.w;
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) red[threadIdx.x * 8 + i] = s[i];
-    __syncthreads();
-    if (tr == 0 && j < cv8) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            float acc = 0.f;
-            for (int r = 0; r < rows; ++r) acc += red[(r * cvb + tc) * 8 + i];
-            const int c = j * 8 + i;
-            if (c < C) atomicAdd(colsum + c, acc);
-        }
-    }
-}
-
-static int split_dy_launch(const effdet_wgrad_args* a, int cout_pad, cudaStream_t st) {
-    const int HW = a->H * a->W;
-    if (!a->dbias) {
-        int blocks = cdiv((long long)a->B * HW * (cout_pad / 8), 256);
-        if (blocks > num_sms() * 16) blocks = num_sms() * 16;
-        split_planes_kernel<<<blocks, 256, 0, st>>>(a->dy, a->dy_bstride, nullptr, (__nv_bfloat16*)a->ws_dy, a->B, HW, a->Cout, cout_pad);
-        return launch_status("split_planes_kernel");
-    }
-    const int cv8 = cout_pad / 8;
-    const int cvb = cv8 < 256 ? cv8 : 256;
-    const int rows = 256 / cvb;
-    const long long nrows = (long long)a->B * HW;
-    long long rpb = (nrows + num_sms() * 4 - 1) / (num_sms() * 4);
-    if (rpb < (long long)rows * 8) rpb = (long long)rows * 8;
-    dim3 grid(cdiv(nrows, rpb), cdiv(cv8, cvb));
-    split_planes_colsum_kernel<<<grid, 256, 0, st>>>(a->dy, a->dy_bstride, (__nv_bfloat16*)a->ws_dy, a->dbias, a->B, HW, a->Cout,
-                                                    cout_pad, (int)rpb);
-    return launch_status("split_planes_colsum_kernel");
-}
-
 // ---------------------------------------------------------------------------------------------
 // weight pre-split: OIHW fp32 -> bf16 planes [2][rows][taps][Kpad] (K-major, zero padded)
 //   forward pack : rows = Cout, k = Cin,  W[n][c][tap]
@@ -727,67 +472,45 @@ __global__ void pack_weight_tc_kernel(const float* __restrict__ w, __nv_bfloat16
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
+EncodeTiledFn encode_fn() {
+    static EncodeTiledFn fn = nullptr;
+    static bool tried = false;
+    if (!tried) {
+        tried = true;
+        void* ptr = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
+            q == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<EncodeTiledFn>(ptr);
+    }
+    return fn;
+}
 
+int conv_tc_kpad(int k) { return (k + kTileK - 1) / kTileK * kTileK; }
 
 bool conv_tc_eligible(const effdet_conv_args* a) {
-    if (a->w_tc == nullptr || a->Cin % 4 || a->Cout % 4 || a->Cout < 16) return false;
-    // the narrowest 1x1 layers stay on the CUDA cores: too little work per tile for the tensor-core pipeline
-    if (a->ksize == 1 && (a->Cin < 24 || (a->Cin <= 32 && a->Cout <= 16))) return false;
-    return true;
+    // the 3x3 convs of neck and head; the MBConv prologue / epilogue inputs are served by the CUDA-core kernel
+    return a->w_tc != nullptr && a->ksize == 3 && a->Cin % 4 == 0 && a->Cout % 4 == 0 && a->Cout >= 16 && !a->a_scale &&
+           !a->z && !a->scale && !a->shift && !a->row_scale && !a->in_scale;
 }
 
-int conv_tc_launch(const effdet_conv_args* a, cudaStream_t st) {
-    EncodeTiledFn enc = encode_fn();
-    if (!enc) return fail(EFFDET_ERR_UNSUPPORTED, "conv2d(tc): cuTensorMapEncodeTiled unavailable");
-    const long long Mll = (long long)a->B * a->H * a->W;
-    const int M = (int)Mll, HW = a->H * a->W;
-    const int taps = a->ksize * a->ksize;
-    const int kpad = conv_tc_kpad(a->Cin);
-    const int kblocks = kpad / kTileK;
-    const int KT = taps * kblocks;
-    // 128 x 128 tiles at most: the accumulator lives in the two warpgroups' registers (64 per thread)
-    const int BN = a->Cout <= 64 ? 64 : 128;
-    CUtensorMap map;
-    const cuuint64_t gdim[3] = {(cuuint64_t)taps * kpad, (cuuint64_t)a->Cout, 2};
-    const cuuint64_t gstr[2] = {(cuuint64_t)taps * kpad * 2, (cuuint64_t)a->Cout * taps * kpad * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)kTileK, (cuuint32_t)BN, 1};
+// 3-D tensor map over K-major bf16 hi/lo planes [2][rows][k]: boxes of 64 k (one 128-byte swizzled row) x box_rows rows
+int kmajor_planes_map(EncodeTiledFn enc, CUtensorMap* map, const void* base, int rows, int k, int box_rows) {
+    const cuuint64_t gdim[3] = {(cuuint64_t)k, (cuuint64_t)rows, 2};
+    const cuuint64_t gstr[2] = {(cuuint64_t)k * 2, (cuuint64_t)rows * k * 2};
+    const cuuint32_t box[3] = {(cuuint32_t)kTileK, (cuuint32_t)box_rows, 1};
     const cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(a->w_tc), gdim, gstr, box, estr,
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim, gstr, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(EFFDET_ERR_LAUNCH, "conv2d(tc): cuTensorMapEncodeTiled failed (%d)", (int)r);
-    dim3 grid(cdiv(M, kTileM), cdiv(a->Cout, BN));
-    const bool mb = a->a_scale || a->z || a->scale || a->row_scale || a->in_scale;
-#define EFFDET_TC_LAUNCH1(BN_, ST_, MB_)                                                                                   \
-    do {                                                                                                                  \
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN_, ST_, MB_>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
-                                             FwdSmem<BN_, ST_>::kBytes);                                                  \
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "conv2d(tc): smem opt-in: %s", cudaGetErrorString(e));       \
-        conv_tc_kernel<BN_, ST_, MB_><<<grid, kFwdThreads, FwdSmem<BN_, ST_>::kBytes, st>>>(map, *a, M, HW, kblocks);      \
-    } while (0)
-#define EFFDET_TC_LAUNCH(BN_, ST_)                                                                                         \
-    do {                                                                                                                  \
-        if (mb) EFFDET_TC_LAUNCH1(BN_, ST_, true);                                                                        \
-        else EFFDET_TC_LAUNCH1(BN_, ST_, false);                                                                          \
-    } while (0)
-    // short reductions (1x1 convs of the backbone): single-stage instances (less shared memory, more CTAs per SM);
-    // long reductions: deep pipelines
-    if (KT <= 2) {
-        if (BN == 64) EFFDET_TC_LAUNCH(64, 1);
-        else EFFDET_TC_LAUNCH(128, 1);
-    } else {
-        if (BN == 64) EFFDET_TC_LAUNCH(64, 4);
-        else EFFDET_TC_LAUNCH(128, 3);
-    }
-#undef EFFDET_TC_LAUNCH
-#undef EFFDET_TC_LAUNCH1
-    return launch_status("conv_tc_kernel");
+    if (r != CUDA_SUCCESS) return fail(EFFDET_ERR_LAUNCH, "tensor map of bf16 planes [2][%d][%d] failed (%d)", rows, k, (int)r);
+    return EFFDET_OK;
 }
 
-
-int conv_tc_multi_launch(const effdet_conv_args* levels, int nlevels, cudaStream_t st) {
+// levels share weights, bias, channels and activation (checked by the caller)
+int conv_tc_launch(const effdet_conv_args* levels, int nlevels, cudaStream_t st) {
     EncodeTiledFn enc = encode_fn();
-    if (!enc) return fail(EFFDET_ERR_UNSUPPORTED, "conv2d_multi(tc): cuTensorMapEncodeTiled unavailable");
+    if (!enc) return fail(EFFDET_ERR_UNSUPPORTED, "conv2d(tc): cuTensorMapEncodeTiled unavailable");
     const effdet_conv_args* a = &levels[0];
     const int taps = a->ksize * a->ksize;
     const int kpad = conv_tc_kpad(a->Cin);
@@ -795,14 +518,8 @@ int conv_tc_multi_launch(const effdet_conv_args* levels, int nlevels, cudaStream
     // 128 x 128 tiles at most: the accumulator lives in the two warpgroups' registers (64 per thread)
     const int BN = a->Cout <= 64 ? 64 : 128;
     CUtensorMap map;
-    const cuuint64_t gdim[3] = {(cuuint64_t)taps * kpad, (cuuint64_t)a->Cout, 2};
-    const cuuint64_t gstr[2] = {(cuuint64_t)taps * kpad * 2, (cuuint64_t)a->Cout * taps * kpad * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)kTileK, (cuuint32_t)BN, 1};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(a->w_tc), gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(EFFDET_ERR_LAUNCH, "conv2d_multi(tc): cuTensorMapEncodeTiled failed (%d)", (int)r);
+    int s = kmajor_planes_map(enc, &map, a->w_tc, a->Cout, taps * kpad, BN);
+    if (s) return s;
     ConvMultiArgs ma;
     memset(&ma, 0, sizeof(ma));
     ma.nlevels = nlevels;
@@ -814,24 +531,16 @@ int conv_tc_multi_launch(const effdet_conv_args* levels, int nlevels, cudaStream
     }
     for (int l = nlevels; l <= kMaxLevels; ++l) ma.tile_begin[l] = tiles;
     dim3 grid(tiles, cdiv(a->Cout, BN));
-#define EFFDET_TCM_LAUNCH(BN_, ST_)                                                                                        \
-    do {                                                                                                                  \
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_multi_kernel<BN_, ST_>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                             FwdSmem<BN_, ST_>::kBytes);                                                  \
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "conv2d_multi(tc): smem opt-in: %s", cudaGetErrorString(e)); \
-        conv_tc_multi_kernel<BN_, ST_><<<grid, kFwdThreads, FwdSmem<BN_, ST_>::kBytes, st>>>(map, ma, kblocks);            \
-    } while (0)
-    if (BN == 64) EFFDET_TCM_LAUNCH(64, 4);
-    else EFFDET_TCM_LAUNCH(128, 3);
-#undef EFFDET_TCM_LAUNCH
-    return launch_status("conv_tc_multi_kernel");
+    if (BN == 64) return launch_smem("conv_tc_kernel", conv_tc_kernel<64, 4>, grid, kTcThreads, FwdSmem<64, 4>::kBytes, st, map, ma, kblocks);
+    return launch_smem("conv_tc_kernel", conv_tc_kernel<128, 3>, grid, kTcThreads, FwdSmem<128, 3>::kBytes, st, map, ma, kblocks);
 }
 
 bool wgrad_tc_eligible(const effdet_wgrad_args* a) {
-    if (a->precision != 1 || a->Cin % 4 || a->Cout % 4 || a->Cin < 16 || a->Cout < 16) return false;
+    // the tensor-core weight gradients have no input prologue: those convs go to the CUDA-core kernel
+    if (a->precision != 1 || a->Cin % 4 || a->Cout % 4 || a->Cin < 16 || a->Cout < 16 || a->a_scale || a->in_scale) return false;
     WgGeom g;
     const bool tma_ok = (a->ws_x || a->x_planes) && (a->ws_dy || a->dy_planes) && wg_geometry(a->B, a->H, a->W, &g);
-    return tma_ok || (!a->a_scale && !a->in_scale && !a->dy_planes && !a->x_planes);     // the gather-producer fallback has no input prologue
+    return tma_ok || (!a->dy_planes && !a->x_planes);     // the gathering kernel reads fp32 operands only
 }
 
 bool wg_geometry(int B, int H, int W, WgGeom* g) {
@@ -865,62 +574,9 @@ int planes_map(EncodeTiledFn enc, CUtensorMap* map, void* base, int B, int H, in
     return EFFDET_OK;
 }
 
-// TMA-fed weight gradient; returns 1 when the geometry has no legal pixel box (caller falls back)
-static int wgrad_tc2_launch(const effdet_wgrad_args* a, cudaStream_t st) {
-    WgGeom g;
-    EncodeTiledFn enc = encode_fn();
-    if (!enc || !(a->ws_x || a->x_planes) || !(a->ws_dy || a->dy_planes) || !wg_geometry(a->B, a->H, a->W, &g)) return 1;
-    const int HW = a->H * a->W;
-    const int cin_pad = conv_tc_kpad(a->Cin), cout_pad = conv_tc_kpad(a->Cout);
-    int s = EFFDET_OK;
-    if (!a->x_planes) {
-        int blocks = cdiv((long long)a->B * HW * (cin_pad / 8), 256);
-        if (blocks > num_sms() * 16) blocks = num_sms() * 16;
-        split_planes_kernel<<<blocks, 256, 0, st>>>(a->x, a->x_bstride, a->a_scale, (__nv_bfloat16*)a->ws_x, a->B, HW, a->Cin, cin_pad,
-                                                    a->in_scale, a->in_shift);
-        s = launch_status("split_planes_kernel");
-        if (s) return s;
-    }
-    CUtensorMap mdy, mx;
-    if (a->dy_planes) {        // dy arrives pre-split (unpadded pitch; TMA zero-fills the channels beyond Cout)
-        if ((s = planes_map(enc, &mdy, const_cast<void*>(a->dy_planes), a->B, a->H, a->W, a->Cout, (a->Cout + 7) / 8 * 8, g))) return s;
-    } else {
-        if ((s = split_dy_launch(a, cout_pad, st))) return s;      // also accumulates the bias gradient
-        if ((s = planes_map(enc, &mdy, a->ws_dy, a->B, a->H, a->W, cout_pad, cout_pad, g))) return s;
-    }
-    if (a->x_planes) {
-        if ((s = planes_map(enc, &mx, const_cast<void*>(a->x_planes), a->B, a->H, a->W, a->Cin, (a->Cin + 7) / 8 * 8, g))) return s;
-    } else {
-        if ((s = planes_map(enc, &mx, a->ws_x, a->B, a->H, a->W, cin_pad, cin_pad, g))) return s;
-    }
-    const int taps = a->ksize * a->ksize;
-    const int BC = a->Cin > 64 ? 256 : 64;
-    const int ctiles = cdiv(a->Cin, BC), ntiles = cdiv(a->Cout, kTileM);
-    const int nchunks = g.nbx * g.nby * g.nbb;
-    // split-K so that the grid is as close as possible to (but not above) two full waves of CTAs
-    int splits = (num_sms() * 2) / (ctiles * ntiles * taps);
-    if (splits < 1) splits = 1;
-    if (splits > cdiv(nchunks, 4)) splits = cdiv(nchunks, 4);
-    int cps = cdiv(nchunks, splits);
-    splits = cdiv(nchunks, cps);
-    dim3 grid(ctiles * ntiles, taps, splits);
-    cudaError_t e;
-    if (BC == 256) {
-        constexpr int ST = 2;
-        e = cudaFuncSetAttribute(wgrad_tc2_kernel<256, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem<256, ST>::kBytes);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad(tc): smem opt-in: %s", cudaGetErrorString(e));
-        wgrad_tc2_kernel<256, ST><<<grid, kTcThreads, WgSmem<256, ST>::kBytes, st>>>(mdy, mx, *a, g, cps, ctiles);
-    } else {
-        constexpr int ST = 4;
-        e = cudaFuncSetAttribute(wgrad_tc2_kernel<64, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem<64, ST>::kBytes);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad(tc): smem opt-in: %s", cudaGetErrorString(e));
-        wgrad_tc2_kernel<64, ST><<<grid, kTcThreads, WgSmem<64, ST>::kBytes, st>>>(mdy, mx, *a, g, cps, ctiles);
-    }
-    return launch_status("wgrad_tc2_kernel");
-}
-
-// all levels in one launch; returns 1 when some level cannot use the TMA path (caller falls back per level)
-int wgrad_tc2_multi_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t st) {
+// TMA-fed weight gradient of one shared-weight layer over all levels in one launch; returns 1 when some level cannot use
+// it (no legal pixel box, no plane workspace, an input prologue) and the caller falls back
+static int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t st) {
     EncodeTiledFn enc = encode_fn();
     if (!enc || nlevels > kWgMaxLevels) return 1;
     WgMaps maps;
@@ -949,19 +605,15 @@ int wgrad_tc2_multi_launch(const effdet_wgrad_args* levels, int nlevels, cudaStr
             if ((s = planes_map(enc, &maps.x[l], const_cast<void*>(a->x_planes), a->B, a->H, a->W, a->Cin, (a->Cin + 7) / 8 * 8, ma.g[l])))
                 return s;
         } else {
-            int blocks = cdiv((long long)a->B * HW * (cin_pad / 8), 256);
-            if (blocks > num_sms() * 16) blocks = num_sms() * 16;
-            split_planes_kernel<<<blocks, 256, 0, st>>>(a->x, a->x_bstride, nullptr, (__nv_bfloat16*)a->ws_x, a->B, HW, a->Cin, cin_pad);
-            s = launch_status("split_planes_kernel");
-            if (s) return s;
+            if ((s = to_planes_launch(a->x, a->x_bstride, nullptr, 0, a->ws_x, nullptr, a->B, HW, a->Cin, cin_pad, st))) return s;
             if ((s = planes_map(enc, &maps.x[l], a->ws_x, a->B, a->H, a->W, cin_pad, cin_pad, ma.g[l]))) return s;
         }
-        if (a->dy_planes) {
+        if (a->dy_planes) {         // unpadded pitch: TMA zero-fills the channels beyond Cout
             if ((s = planes_map(enc, &maps.dy[l], const_cast<void*>(a->dy_planes), a->B, a->H, a->W, a->Cout, (a->Cout + 7) / 8 * 8,
                                 ma.g[l])))
                 return s;
-        } else {
-            if ((s = split_dy_launch(a, cout_pad, st))) return s;  // also accumulates the bias gradient
+        } else {                    // the split pass also accumulates the bias gradient
+            if ((s = to_planes_launch(a->dy, a->dy_bstride, nullptr, 0, a->ws_dy, a->dbias, a->B, HW, a->Cout, cout_pad, st))) return s;
             if ((s = planes_map(enc, &maps.dy[l], a->ws_dy, a->B, a->H, a->W, cout_pad, cout_pad, ma.g[l]))) return s;
         }
     }
@@ -969,34 +621,24 @@ int wgrad_tc2_multi_launch(const effdet_wgrad_args* levels, int nlevels, cudaStr
     const int taps = a0->ksize * a0->ksize;
     const int BC = a0->Cin > 64 ? 256 : 64;
     const int ctiles = cdiv(a0->Cin, BC), ntiles = cdiv(a0->Cout, kTileM);
+    // split-K so that the grid is as close as possible to (but not above) two full waves of CTAs
     int splits = (num_sms() * 2) / (ctiles * ntiles * taps);
     if (splits < 1) splits = 1;
     if (splits > cdiv(chunks, 4)) splits = cdiv(chunks, 4);
     int cps = cdiv(chunks, splits);
     splits = cdiv(chunks, cps);
-    cudaError_t e;
     dim3 grid(ctiles * ntiles, taps, splits);
-    if (BC == 256) {
-        constexpr int ST = 2;
-        e = cudaFuncSetAttribute(wgrad_tc2_multi_kernel<256, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem<256, ST>::kBytes);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad_multi(tc): smem opt-in: %s", cudaGetErrorString(e));
-        wgrad_tc2_multi_kernel<256, ST><<<grid, kTcThreads, WgSmem<256, ST>::kBytes, st>>>(maps, ma, cps, ctiles);
-    } else {
-        constexpr int ST = 4;
-        e = cudaFuncSetAttribute(wgrad_tc2_multi_kernel<64, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem<64, ST>::kBytes);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad_multi(tc): smem opt-in: %s", cudaGetErrorString(e));
-        wgrad_tc2_multi_kernel<64, ST><<<grid, kTcThreads, WgSmem<64, ST>::kBytes, st>>>(maps, ma, cps, ctiles);
-    }
-    return launch_status("wgrad_tc2_multi_kernel");
+    if (BC == 256)
+        return launch_smem("wgrad_tc2_multi_kernel", wgrad_tc2_multi_kernel<256, 2>, grid, kTcThreads, WgSmem<256, 2>::kBytes, st,
+                           maps, ma, cps, ctiles);
+    return launch_smem("wgrad_tc2_multi_kernel", wgrad_tc2_multi_kernel<64, 4>, grid, kTcThreads, WgSmem<64, 4>::kBytes, st, maps,
+                       ma, cps, ctiles);
 }
 
 int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st, bool* dbias_done) {
-    *dbias_done = false;
-    {
-        const int r = wgrad_tc2_launch(a, st);
-        if (r == 0) *dbias_done = true;     // the TMA path folds the bias gradient into its dy split pass
-        if (r <= 0) return r;       // launched (0) or failed (<0); 1 = geometry unsupported -> gather kernel
-    }
+    const int r = wgrad_tc2_launch(a, 1, st);
+    *dbias_done = r == 0;       // the TMA path folds the bias gradient into its dy split pass
+    if (r <= 0) return r;       // launched (0) or failed (<0); 1 = geometry unsupported -> gather kernel
     const long long Mll = (long long)a->B * a->H * a->W;
     const int M = (int)Mll, HW = a->H * a->W;
     const int taps = a->ksize * a->ksize;
@@ -1009,19 +651,10 @@ int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st, bool* dbias_don
     int cps = cdiv(nchunks, splits);
     splits = cdiv(nchunks, cps);
     dim3 grid(ctiles * ntiles, taps, splits);
-    cudaError_t e;
-    if (BC == 256) {
-        constexpr int ST = 2;
-        e = cudaFuncSetAttribute(wgrad_tc_kernel<256, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem<256, ST>::kBytes);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad(tc): smem opt-in: %s", cudaGetErrorString(e));
-        wgrad_tc_kernel<256, ST><<<grid, kTcProducers, WgSmem<256, ST>::kBytes, st>>>(*a, M, HW, cps, ctiles);
-    } else {
-        constexpr int ST = 4;
-        e = cudaFuncSetAttribute(wgrad_tc_kernel<64, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem<64, ST>::kBytes);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad(tc): smem opt-in: %s", cudaGetErrorString(e));
-        wgrad_tc_kernel<64, ST><<<grid, kTcProducers, WgSmem<64, ST>::kBytes, st>>>(*a, M, HW, cps, ctiles);
-    }
-    return launch_status("wgrad_tc_kernel");
+    if (BC == 256)
+        return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<256, 2>, grid, kTcProducers, WgSmem<256, 2>::kBytes, st, *a, M, HW, cps,
+                           ctiles);
+    return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<64, 4>, grid, kTcProducers, WgSmem<64, 4>::kBytes, st, *a, M, HW, cps, ctiles);
 }
 
 }  // namespace effdet
@@ -1034,11 +667,6 @@ extern "C" int effdet_wgrad_tc_geometry_ok(int B, int H, int W) {
     return wg_geometry(B, H, W, &g) ? 1 : 0;
 }
 
-namespace effdet {   // defined in conv_simt.cu
-int colsum_launch(const float* x, float* out, long long M, int N, long long HW, long long bstride, int device,
-                  effdet_stream_t stream);
-}
-
 extern "C" int effdet_conv2d_wgrad_multi(const effdet_wgrad_args* levels, int nlevels, int device, effdet_stream_t stream) {
     EFFDET_REQUIRE(levels && nlevels >= 1, "conv2d_wgrad_multi: no levels");
     bool same = true;
@@ -1049,9 +677,9 @@ extern "C" int effdet_conv2d_wgrad_multi(const effdet_wgrad_args* levels, int nl
         same = same && a->dw == levels[0].dw && a->dbias == levels[0].dbias && a->Cin == levels[0].Cin &&
                a->Cout == levels[0].Cout && a->ksize == levels[0].ksize && a->precision == 1 && wgrad_tc_eligible(a);
     }
-    if (same && nlevels > 1) {
+    if (same && nlevels > 1) {          // one level: effdet_conv2d_wgrad checks its arguments and takes the same kernel
         EFFDET_DEVICE(device);
-        const int r = wgrad_tc2_multi_launch(levels, nlevels, (cudaStream_t)stream);
+        const int r = wgrad_tc2_launch(levels, nlevels, (cudaStream_t)stream);
         if (r < 0) return r;
         if (r == 0) return EFFDET_OK;          // bias gradient was fused into the dy split pass
     }
@@ -1072,15 +700,14 @@ extern "C" int effdet_conv2d_multi(const effdet_conv_args* levels, int nlevels, 
                            a->act == levels[0].act && a->w == levels[0].w && a->w_tc == levels[0].w_tc &&
                            a->bias == levels[0].bias,
                        "conv2d_multi: all levels must share weights, bias, channels and activation");
-        const bool mb = a->a_scale || a->z || a->scale || a->row_scale || a->in_scale;
-        tc = tc && conv_tc_eligible(a) && !mb && (long long)a->B * a->H * a->W < (1ll << 31);
+        tc = tc && conv_tc_eligible(a) && (long long)a->B * a->H * a->W < (1ll << 31);
         EFFDET_REQUIRE(aligned16(a->x) && aligned16(a->y) && aligned16(a->residual) && aligned16(a->mask_src) &&
                            a->x_bstride % 4 == 0 && a->y_bstride % 4 == 0 && a->r_bstride % 4 == 0 && a->m_bstride % 4 == 0,
                        "conv2d_multi: alignment");
     }
-    if (tc && nlevels > 1) {
+    if (tc && nlevels > 1) {          // one level: effdet_conv2d checks its arguments and takes the same kernel
         EFFDET_DEVICE(device);
-        return conv_tc_multi_launch(levels, nlevels, (cudaStream_t)stream);
+        return conv_tc_launch(levels, nlevels, (cudaStream_t)stream);
     }
     for (int l = 0; l < nlevels; ++l) {          // exact-fp32 mode / unsupported shapes: one launch per level
         int s = effdet_conv2d(&levels[l], device, stream);

@@ -20,8 +20,6 @@
 // BIFPN lateral convs (models/bifpn.py:96-105).
 #include "tc_ptx.cuh"
 
-#include <stdlib.h>
-
 namespace effdet {
 
 constexpr int kPwA32Half = 128 * 128;      // bytes of one fp32 half-box: 128 rows x 32 floats
@@ -292,16 +290,8 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     }
 }
 
-static bool pw_enabled() {
-    static const bool on = [] {
-        const char* v = getenv("EFFDET_B200_PW");
-        return !(v && v[0] == '0');
-    }();
-    return on;
-}
-
 bool pw_gemm_eligible(const effdet_conv_args* a) {
-    if (!pw_enabled() || a->ksize != 1 || a->w_tc == nullptr || a->Cin % 4 || a->Cout % 4 || a->Cin < 8 || a->Cout < 8) return false;
+    if (a->ksize != 1 || a->w_tc == nullptr || a->Cin % 4 || a->Cout % 4 || a->Cin < 8 || a->Cout < 8) return false;
     const long long HW = (long long)a->H * a->W;
     if (a->x_planes) return a->Cin % 8 == 0 && !a->in_scale && !a->a_scale && (long long)a->B * HW < (1ll << 31);
     if (a->x_bstride != HW * a->Cin) return false;              // x must be one dense [M, Cin] matrix for the 2-D tensor map
@@ -340,14 +330,8 @@ int pw_gemm_launch(const effdet_conv_args* a, cudaStream_t st) {
 
     CUtensorMap map_a, map_b;
     if (P.planes) {
-        const cuuint64_t gdim[3] = {(cuuint64_t)a->Cin, (cuuint64_t)P.M, 2};
-        const cuuint64_t gstr[2] = {(cuuint64_t)a->Cin * 2, (cuuint64_t)P.M * a->Cin * 2};
-        const cuuint32_t box[3] = {64, 128, 1};
-        const cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&map_a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(a->x_planes), gdim, gstr, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return fail(EFFDET_ERR_LAUNCH, "conv2d(pw): tensor map of the x planes failed (%d)", (int)r);
+        const int s = kmajor_planes_map(enc, &map_a, a->x_planes, P.M, a->Cin, 128);
+        if (s) return s;
     } else {
         const cuuint64_t gdim[2] = {(cuuint64_t)a->Cin, (cuuint64_t)P.M};
         const cuuint64_t gstr[1] = {(cuuint64_t)a->Cin * 4};
@@ -358,28 +342,11 @@ int pw_gemm_launch(const effdet_conv_args* a, cudaStream_t st) {
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return fail(EFFDET_ERR_LAUNCH, "conv2d(pw): tensor map of x failed (%d)", (int)r);
     }
-    {
-        const cuuint64_t gdim[3] = {(cuuint64_t)kpad, (cuuint64_t)a->Cout, 2};
-        const cuuint64_t gstr[2] = {(cuuint64_t)kpad * 2, (cuuint64_t)a->Cout * kpad * 2};
-        const cuuint32_t box[3] = {64, (cuuint32_t)P.BN, 1};
-        const cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(a->w_tc), gdim, gstr, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return fail(EFFDET_ERR_LAUNCH, "conv2d(pw): tensor map of the weights failed (%d)", (int)r);
-    }
+    const int s = kmajor_planes_map(enc, &map_b, a->w_tc, a->Cout, kpad, P.BN);
+    if (s) return s;
     const int grid = P.units < num_sms() ? P.units : num_sms();
-    cudaError_t e;
-    if (P.BN == 128) {
-        e = cudaFuncSetAttribute(pw_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "conv2d(pw): smem opt-in: %s", cudaGetErrorString(e));
-        pw_gemm_kernel<2><<<grid, kPwThreads, smem, st>>>(map_a, map_b, P);
-    } else {
-        e = cudaFuncSetAttribute(pw_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "conv2d(pw): smem opt-in: %s", cudaGetErrorString(e));
-        pw_gemm_kernel<1><<<grid, kPwThreads, smem, st>>>(map_a, map_b, P);
-    }
-    return launch_status("pw_gemm_kernel");
+    if (P.BN == 128) return launch_smem("pw_gemm_kernel", pw_gemm_kernel<2>, grid, kPwThreads, smem, st, map_a, map_b, P);
+    return launch_smem("pw_gemm_kernel", pw_gemm_kernel<1>, grid, kPwThreads, smem, st, map_a, map_b, P);
 }
 
 }  // namespace effdet

@@ -1,9 +1,9 @@
 // Weight gradient of the 1x1 convolutions of the MBConv block (models/efficientnet.py:85 expand, :96 project; reached
 // through autograd's cuDNN bwd-filter in the reference), straight from the fp32 tensors:
 //     dW[n][c] += sum_m dy[m][n] * xt[m][c],      xt = swish(x*in_scale+in_shift) * a_scale[image]   (both optional)
-// The TMA-fed kernel in conv_tc.cu wants both operands pre-split into bf16 hi/lo planes; for these layers that cost a
-// split pass over x (with the BN+swish+SE-gate prologue) and one over dy -- each a full read + write of an expanded
-// activation -- before the GEMM read them a third time.  Here eight converter warps read the fp32 rows with 128-bit
+// The TMA-fed kernel in conv_tc.cu wants both operands pre-split into bf16 hi/lo planes; for these layers that would
+// cost a split pass over x (after the BN+swish+SE-gate prologue) and one over dy -- each a full read + write of an
+// expanded activation -- before the GEMM read them a third time.  Here eight converter warps read the fp32 rows with 128-bit
 // coalesced loads, apply the prologue in registers, split to bf16 hi/lo and write the operand tiles in the
 // SWIZZLE_128B "MN-major" layout (row = pixel, 128 bytes = 64 channels) the tensor-map loads would have produced; two
 // consumer warpgroups (64 output channels each) issue the bf16x3 wgmma (GEMM-K = pixels, M = output channels, N = input
@@ -11,7 +11,6 @@
 // once: algorithmic bytes = 4*M*(Cin + Cout) (dy pre-split by the depthwise backward kernel: same 4 bytes / element).
 #include "tc_ptx.cuh"
 
-#include <cstdlib>
 #include <cstring>
 
 namespace effdet {
@@ -225,17 +224,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) pw_wgrad_kernel(const __grid_co
     }
 }
 
-static bool pw_wgrad_enabled() {
-    static int on = -1;
-    if (on < 0) {
-        const char* e = getenv("EFFDET_B200_PWWG");
-        on = (e && e[0] == '0') ? 0 : 1;
-    }
-    return on;
-}
-
 bool pw_wgrad_eligible(const effdet_wgrad_args* a) {
-    if (!pw_wgrad_enabled() || a->ksize != 1 || a->precision != 1 || a->dbias || a->x_planes || !a->x) return false;
+    if (a->ksize != 1 || a->precision != 1 || a->dbias || a->x_planes || !a->x) return false;
     if (a->Cin % 8 || a->Cout % 8 || a->Cin < 8 || a->Cout < 8) return false;
     const long long HW = (long long)a->H * a->W;
     if (a->x_bstride != HW * a->Cin) return false;
@@ -285,17 +275,8 @@ int pw_wgrad_launch(const effdet_wgrad_args* a, cudaStream_t st) {
     P.NS = (200 * 1024) / P.stage_bytes;
     if (P.NS > 4) P.NS = 4;
     const size_t smem = (size_t)P.NS * P.stage_bytes + 128 + 2 * 256 * sizeof(float) + 1024;
-    cudaError_t e;
-    if (P.NX > 64) {
-        e = cudaFuncSetAttribute(pw_wgrad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad(pw): smem opt-in: %s", cudaGetErrorString(e));
-        pw_wgrad_kernel<2><<<dim3(tiles, splits), kWgThreads, smem, st>>>(P);
-    } else {
-        e = cudaFuncSetAttribute(pw_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad(pw): smem opt-in: %s", cudaGetErrorString(e));
-        pw_wgrad_kernel<1><<<dim3(tiles, splits), kWgThreads, smem, st>>>(P);
-    }
-    return launch_status("pw_wgrad_kernel");
+    if (P.NX > 64) return launch_smem("pw_wgrad_kernel", pw_wgrad_kernel<2>, dim3(tiles, splits), kWgThreads, smem, st, P);
+    return launch_smem("pw_wgrad_kernel", pw_wgrad_kernel<1>, dim3(tiles, splits), kWgThreads, smem, st, P);
 }
 
 }  // namespace effdet

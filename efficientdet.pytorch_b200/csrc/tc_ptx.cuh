@@ -233,6 +233,23 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn encode_fn();      // cuTensorMapEncodeTiled through the runtime's driver entry point table (conv_tc.cu)
 int conv_tc_kpad(int k);
+// 3-D tensor map over K-major bf16 hi/lo planes [2][rows][k] (the weight packs, the x planes of a 1x1 conv): boxes of
+// 64 k x box_rows rows, SWIZZLE_128B (conv_tc.cu)
+int kmajor_planes_map(EncodeTiledFn enc, CUtensorMap* map, const void* base, int rows, int k, int box_rows);
+// fp32 [B][HW][C] (image stride x_bstride) -> bf16 hi/lo planes [2][B*HW][pitch] with zero padded channels; optionally
+// times p*(1-p) of prob, optionally accumulating the per-channel column sums into colsum (conv_planes.cu)
+int to_planes_launch(const float* x, long long x_bstride, const float* prob, long long p_bstride, void* out, float* colsum,
+                     int B, int HW, int C, int pitch, cudaStream_t st);
+
+// Opts the kernel in to `smem` bytes of dynamic shared memory (the tensor-core kernels need more than the default
+// 48 KB), launches it and returns the launch status under `name`.
+template <class... P, class... A>
+int launch_smem(const char* name, void (*kernel)(P...), dim3 grid, int threads, size_t smem, cudaStream_t st, const A&... args) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "%s: smem opt-in: %s", name, cudaGetErrorString(e));
+    kernel<<<grid, threads, smem, st>>>(args...);
+    return launch_status(name);
+}
 
 // Pixel boxes of the TMA-fed kernels: a [B,H,W,*] map is tiled into boxes of Wb x Hb x Bb = kstage pixels (16..64, a
 // multiple of 16) that one tensor-map load turns into kstage consecutive 128-byte rows of shared memory (conv_tc.cu)

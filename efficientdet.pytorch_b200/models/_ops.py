@@ -597,8 +597,8 @@ class BiFPNLayerFn(torch.autograd.Function):
 
         # tensor-core mode: the fused map is written as bf16 hi/lo planes and the node conv is the TMA-fed planes
         # kernel (no gather, no split pass in the weight gradient); every level must admit a TMA pixel box
-        pl = (tc_enabled() and C % 4 == 0 and os.environ.get('EFFDET_B200_BIFPN_PLANES', '1') != '0' and
-              all(N.load().effdet_wgrad_tc_geometry_ok(t.shape[0], t.shape[1], t.shape[2]) for t in ins))
+        pl = tc_enabled() and C % 4 == 0 and all(N.load().effdet_wgrad_tc_geometry_ok(t.shape[0], t.shape[1], t.shape[2])
+                                                 for t in ins)
 
         def conv(idx, f, like):
             if pl:
@@ -839,7 +839,7 @@ def wgrad_planes_multi(dev_t, levels, dw, Cin, Cout, k):
 
 def head_planes_ok(feats, params):
     """can the RetinaHead run with activations kept as bf16 hi/lo planes (TMA-fed tensor-core path)?"""
-    if not tc_enabled() or os.environ.get('EFFDET_B200_HEAD_PLANES', '1') == '0':
+    if not tc_enabled():
         return False
     lib = N.load()
     for f in feats:
