@@ -14,7 +14,7 @@
 //   warp 8      TMA producer (activation boxes hi/lo + weight tile hi/lo -> mbarrier complete_tx), ring of stages that
 //               runs ahead into the next unit while the consumers are in their epilogue
 //   warps 0-7   two consumer warpgroups, one per 64-row half of the tile: 3 wgmma per K16 (lo*hi, hi*lo, hi*hi) with the
-//               accumulator in registers, then the epilogue: bias / ReLU / sigmoid / ReLU-mask / residual -> bf16 hi/lo
+//               accumulator in registers (single-pass instance, NP = 1: hi*hi only, and the producer loads no lo plane), then the epilogue: bias / ReLU / sigmoid / ReLU-mask / residual -> bf16 hi/lo
 //               planes (the next layer's operand) and / or fp32 (head outputs, data gradient w.r.t. the BiFPN features);
 //               optional per-channel column sums of what was stored (= the bias gradient of the producing layer)
 //               reduced by warp shuffles, one atomic per column per warp
@@ -60,7 +60,8 @@ struct PlMaps {
     CUtensorMap x[kPlMaxLevels];
 };
 
-template <int BN>
+// NP = bf16 products per multiply-add: 3 (split precision) or 1 (hi planes only)
+template <int BN, int NP>
 __global__ void __launch_bounds__(kPlThreads, 1)
 conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ CUtensorMap wmap, const __grid_constant__ PlArgs P) {
     constexpr int kPlBN = BN, kPlStages = PlCfg<BN>::kStages, kPlB = PlCfg<BN>::kB, kPlStage = PlCfg<BN>::kStage;
@@ -111,7 +112,7 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                     mbar_wait(&empty_bar[s], ph ^ 1);
                     uint8_t* a_hi = smem + s * kPlStage;
                     uint8_t* b_hi = a_hi + 2 * kPlA;
-                    mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(2 * nvalid * ks * 128 + 2 * kPlB));
+                    mbar_arrive_expect_tx(&full_bar[s], (uint32_t)((NP == 3 ? 2 : 1) * (nvalid * ks * 128 + kPlB)));
                     for (int q = 0; q < nvalid; ++q) {
                         int ch = box0 + q;
                         const int bx = ch % L.g.nbx;
@@ -120,10 +121,10 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                         const int bb = ch / L.g.nby;
                         const int x0 = bx * L.g.Wb + dx, y0 = by * L.g.Hb + dy, b0 = bb * L.g.Bb;
                         tma_load_5d(a_hi + q * ks * 128, &maps.x[l], &full_bar[s], kb * 64, x0, y0, b0, 0);
-                        tma_load_5d(a_hi + kPlA + q * ks * 128, &maps.x[l], &full_bar[s], kb * 64, x0, y0, b0, 1);
+                        if (NP == 3) tma_load_5d(a_hi + kPlA + q * ks * 128, &maps.x[l], &full_bar[s], kb * 64, x0, y0, b0, 1);
                     }
                     tma_load_3d(b_hi, &wmap, &full_bar[s], kt * 64, n0, 0);
-                    tma_load_3d(b_hi + kPlB, &wmap, &full_bar[s], kt * 64, n0, 1);
+                    if (NP == 3) tma_load_3d(b_hi + kPlB, &wmap, &full_bar[s], kt * 64, n0, 1);
                 }
             }
         }
@@ -150,7 +151,7 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
-                    wg_mma3<NB, 0>(d, sa + k * 32, sa + kPlA + k * 32, sb + k * 32, sb + kPlB + k * 32, 16, 1024, (kt | k) != 0);
+                    wg_mma<NB, 0, NP>(d, sa + k * 32, sa + kPlA + k * 32, sb + k * 32, sb + kPlB + k * 32, 16, 1024, (kt | k) != 0);
                 wgmma_commit();
                 wgmma_wait<1>();                                   // the previous stage is no longer read
                 if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kPlStages]);
@@ -365,6 +366,10 @@ extern "C" int effdet_to_planes(const float* x, int64_t x_bstride, const float* 
 extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, int nlevels, int device, effdet_stream_t stream) {
     EFFDET_REQUIRE(levels && nlevels >= 1 && nlevels <= kPlMaxLevels, "conv_planes_multi: 1..%d levels", kPlMaxLevels);
     const effdet_conv_planes_args* a0 = &levels[0];
+    EFFDET_REQUIRE(!a0->tc_single || a0->ksize == 3, "conv_planes_multi: tc_single is defined for 3x3 convolutions only (ksize %d)",
+                   a0->ksize);
+    for (int l = 1; l < nlevels; ++l)
+        EFFDET_REQUIRE(levels[l].tc_single == a0->tc_single, "conv_planes_multi: levels disagree on tc_single");
     EFFDET_REQUIRE(a0->w_tc && (a0->ksize == 1 || a0->ksize == 3) && a0->Cin % 4 == 0 && a0->Cout % 4 == 0 && a0->Cin >= 8 &&
                        a0->Cout >= 8,
                    "conv_planes_multi: needs the bf16 weight pack, k in {1,3}, channels %% 4 == 0");
@@ -421,6 +426,10 @@ extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, i
     P.colsum = a0->colsum;
     const int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
     cudaStream_t st = (cudaStream_t)stream;
-    if (BN == 64) return launch_smem("conv_planes_kernel", conv_planes_kernel<64>, grid, kPlThreads, PlCfg<64>::kSmem, st, maps, wmap, P);
-    return launch_smem("conv_planes_kernel", conv_planes_kernel<128>, grid, kPlThreads, PlCfg<128>::kSmem, st, maps, wmap, P);
+    if (a0->tc_single) {
+        if (BN == 64) return launch_smem("conv_planes_kernel", conv_planes_kernel<64, 1>, grid, kPlThreads, PlCfg<64>::kSmem, st, maps, wmap, P);
+        return launch_smem("conv_planes_kernel", conv_planes_kernel<128, 1>, grid, kPlThreads, PlCfg<128>::kSmem, st, maps, wmap, P);
+    }
+    if (BN == 64) return launch_smem("conv_planes_kernel", conv_planes_kernel<64, 3>, grid, kPlThreads, PlCfg<64>::kSmem, st, maps, wmap, P);
+    return launch_smem("conv_planes_kernel", conv_planes_kernel<128, 3>, grid, kPlThreads, PlCfg<128>::kSmem, st, maps, wmap, P);
 }

@@ -377,6 +377,8 @@ extern "C" int effdet_conv2d(const effdet_conv_args* a, int device, effdet_strea
     EFFDET_REQUIRE(!a->x_planes || (pw_gemm_eligible(a) && aligned16(a->x_planes)),
                    "conv2d: x_planes is only understood by the tensor-core 1x1 path (Cin %% 8 == 0, no input prologue)");
     EFFDET_REQUIRE(a->ksize == 1 || a->ksize == 3, "conv2d: ksize %d not in {1,3}", a->ksize);
+    EFFDET_REQUIRE(!a->tc_single || a->w_tc, "conv2d: tc_single needs the tensor-core weight pack w_tc (the exact-fp32 path has one product)");
+    EFFDET_REQUIRE(!a->tc_single || a->ksize == 3, "conv2d: tc_single is defined for 3x3 convolutions only (ksize %d)", a->ksize);
     EFFDET_REQUIRE(a->Cin % 4 == 0 && a->Cout % 4 == 0, "conv2d: Cin=%d Cout=%d must be multiples of 4", a->Cin, a->Cout);
     EFFDET_REQUIRE(a->B > 0 && a->H > 0 && a->W > 0, "conv2d: empty shape");
     EFFDET_REQUIRE((a->scale == nullptr) == (a->shift == nullptr), "conv2d: scale/shift must come together");
@@ -441,6 +443,8 @@ extern "C" int effdet_conv2d_wgrad(const effdet_wgrad_args* a, int device, effde
                                     (a->ws_dy || a->dy_planes)),
                    "wgrad: x_planes needs precision 1 and no input prologue");
     EFFDET_REQUIRE(a->ksize == 1 || a->ksize == 3, "wgrad: ksize %d not in {1,3}", a->ksize);
+    EFFDET_REQUIRE(!a->tc_single || a->precision == 1, "wgrad: tc_single needs precision 1 (the exact-fp32 path has one product)");
+    EFFDET_REQUIRE(!a->tc_single || a->ksize == 3, "wgrad: tc_single is defined for 3x3 convolutions only (ksize %d)", a->ksize);
     EFFDET_REQUIRE(a->Cin % 4 == 0 && a->Cout % 4 == 0, "wgrad: channels must be multiples of 4");
     EFFDET_REQUIRE(aligned16(a->x) && aligned16(a->dy) && aligned16(a->a_scale) && aligned16(a->in_scale) && aligned16(a->in_shift),
                    "wgrad: pointers must be 16-byte aligned");

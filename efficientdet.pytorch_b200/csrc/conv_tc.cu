@@ -11,7 +11,8 @@
 // bf16 hi + bf16 lo (x = hi + lo to 16 mantissa bits); every product is evaluated as
 //   hi*hi + lo*hi + hi*lo      (three bf16 wgmma, fp32 accumulation in registers)
 // which is ~2^-16 per product -- far inside north_star's 1e-3 where single-pass TF32 is not
-// (SURVEY.md H1) -- at 2/3 the cost of 3xTF32.
+// (SURVEY.md H1) -- at 2/3 the cost of 3xTF32.  Every kernel also has a single-pass instance (template
+// argument NP = 1, the tc_single flag of the C ABI): hi*hi only, the lo halves are neither formed nor loaded.
 //
 // Structure per CTA (288 threads, one 128 x BN output tile):
 //   warps 0-7  two warpgroups: gather the im2col A tile (128 pixels x 64 channels of one tap)
@@ -49,19 +50,20 @@ struct FwdSmem {
 // levels (a handful of CTAs each) ride along with the large ones instead of paying their own latency-bound launch.
 constexpr int kMaxLevels = 8;
 struct ConvMultiArgs {
-    effdet_conv_args lv[kMaxLevels];
+    ConvLevel lv[kMaxLevels];
     int tile_begin[kMaxLevels + 1];
     int nlevels;
 };
 
-template <int BN, int STAGES>
+// NP = bf16 products per multiply-add: 3 (split precision) or 1 (hi only)
+template <int BN, int STAGES, int NP>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ ConvMultiArgs ma, const int kblocks) {
     using S = FwdSmem<BN, STAGES>;
     const int tile = blockIdx.x;
     int l = 0;
     while (l + 1 < ma.nlevels && tile >= ma.tile_begin[l + 1]) ++l;
-    const effdet_conv_args& p = ma.lv[l];
+    const effdet_conv_args& p = ma.lv[l].get();
     const int M = p.B * p.H * p.W, HW = p.H * p.W;
     const int m0 = (tile - ma.tile_begin[l]) * kTileM, n0 = blockIdx.y * BN;
     extern __shared__ uint8_t smem_raw[];
@@ -143,11 +145,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int r = i * 32 + (t >> 3);
-                uint4 hi, lo;
-                split8(v[2 * i], v[2 * i + 1], hi, lo);
                 const int off = r * 128 + ((j ^ (r & 7)) << 4);
-                *reinterpret_cast<uint4*>(a_hi + off) = hi;
-                *reinterpret_cast<uint4*>(a_lo + off) = lo;
+                if constexpr (NP == 3) {
+                    uint4 hi, lo;
+                    split8(v[2 * i], v[2 * i + 1], hi, lo);
+                    *reinterpret_cast<uint4*>(a_hi + off) = hi;
+                    *reinterpret_cast<uint4*>(a_lo + off) = lo;
+                } else {
+                    *reinterpret_cast<uint4*>(a_hi + off) = hi8(v[2 * i], v[2 * i + 1]);
+                }
             }
             fence_proxy_async();
             named_bar_sync(1, kTcProducers);     // the A tile is complete
@@ -157,7 +163,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < kTileK / 16; ++k)
-                wg_mma3<NB, 0>(d, sa + k * 32, sa + S::kA + k * 32, sb + k * 32, sb + S::kB + k * 32, 16, 1024, (kt | k) != 0);
+                wg_mma<NB, 0, NP>(d, sa + k * 32, sa + S::kA + k * 32, sb + k * 32, sb + S::kB + k * 32, 16, 1024, (kt | k) != 0);
             wgmma_commit();
         }
         wgmma_wait<0>();
@@ -214,9 +220,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__
                 const uint32_t ph = (kt / STAGES) & 1;
                 mbar_wait(&empty_bar[s], ph ^ 1);
                 uint8_t* b_hi = smem + s * S::kStage + 2 * S::kA;
-                mbar_arrive_expect_tx(&full_bar[s], 2 * S::kB);
+                mbar_arrive_expect_tx(&full_bar[s], (NP == 3 ? 2 : 1) * S::kB);
                 tma_load_3d(b_hi, &wmap, &full_bar[s], kt * kTileK, n0, 0);
-                tma_load_3d(b_hi + S::kB, &wmap, &full_bar[s], kt * kTileK, n0, 1);
+                if (NP == 3) tma_load_3d(b_hi + S::kB, &wmap, &full_bar[s], kt * kTileK, n0, 1);
             }
         }
     }
@@ -237,8 +243,8 @@ struct WgSmem {
     static constexpr int kBytes = STAGES * kStage + 1024 + 256;
 };
 
-// gather `ngroups` channel groups (64 channels each) of 64 pixel rows into swizzled bf16 planes
-template <int NGROUPS>
+// gather `ngroups` channel groups (64 channels each) of 64 pixel rows into swizzled bf16 planes (NP = 1: hi plane only)
+template <int NGROUPS, int NP>
 __device__ __forceinline__ void wg_produce(const float* __restrict__ src, const long long bstride, const int C, const int c0,
                                            const int H, const int W, const int HW, const int M, const int mbase, const int dy,
                                            const int dx, uint8_t* hi_plane, uint8_t* lo_plane, const int t) {
@@ -264,11 +270,16 @@ __device__ __forceinline__ void wg_produce(const float* __restrict__ src, const 
                 if (c + 4 < C) v1 = ldg4(q + 4);
             }
         }
-        uint4 hi, lo;
-        split8(v0, v1, hi, lo);
-        const int off = g * (kTileK * 128) + r * 128 + ((j ^ (r & 7)) << 4);
-        *reinterpret_cast<uint4*>(hi_plane + off) = hi;
-        *reinterpret_cast<uint4*>(lo_plane + off) = lo;
+        if constexpr (NP == 3) {
+            uint4 hi, lo;
+            split8(v0, v1, hi, lo);
+            const int off = g * (kTileK * 128) + r * 128 + ((j ^ (r & 7)) << 4);
+            *reinterpret_cast<uint4*>(hi_plane + off) = hi;
+            *reinterpret_cast<uint4*>(lo_plane + off) = lo;
+        } else {
+            const int off = g * (kTileK * 128) + r * 128 + ((j ^ (r & 7)) << 4);
+            *reinterpret_cast<uint4*>(hi_plane + off) = hi8(v0, v1);
+        }
     }
 }
 
@@ -288,10 +299,11 @@ __device__ __forceinline__ void wg_atomic_dw(const float (&d)[NB][32], float* dw
         }
 }
 
-template <int BC, int STAGES>
+template <int BC, int STAGES, int NP>
 __global__ void __launch_bounds__(kTcProducers, 1)
-wgrad_tc_kernel(const effdet_wgrad_args p, const int M, const int HW, const int chunks_per_split, const int ctiles) {
+wgrad_tc_kernel(const __grid_constant__ WgradPrefix pa, const int M, const int HW, const int chunks_per_split, const int ctiles) {
     using S = WgSmem<BC, STAGES>;
+    const effdet_wgrad_args& p = pa.get();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1024-byte aligned AND still a shared-space pointer (LDS/STS, not generic LD/ST)
 
@@ -316,12 +328,12 @@ wgrad_tc_kernel(const effdet_wgrad_args p, const int M, const int HW, const int 
         uint8_t* a_hi = smem + s * S::kStage;
         uint8_t* b_hi = a_hi + 2 * S::kA;
         const int mbase = (ch_begin + kt) * kTileK;
-        wg_produce<kTileM / 64>(p.dy, p.dy_bstride, p.Cout, n0, p.H, p.W, HW, M, mbase, 0, 0, a_hi, a_hi + S::kA, t);
-        wg_produce<BC / 64>(p.x, p.x_bstride, p.Cin, c0, p.H, p.W, HW, M, mbase, dy, dx, b_hi, b_hi + S::kB, t);
+        wg_produce<kTileM / 64, NP>(p.dy, p.dy_bstride, p.Cout, n0, p.H, p.W, HW, M, mbase, 0, 0, a_hi, a_hi + S::kA, t);
+        wg_produce<BC / 64, NP>(p.x, p.x_bstride, p.Cin, c0, p.H, p.W, HW, M, mbase, dy, dx, b_hi, b_hi + S::kB, t);
         fence_proxy_async();
         named_bar_sync(1, kTcProducers);
         const uint32_t sa = smem_u32(a_hi) + g * GROUP, sb = smem_u32(b_hi);
-        wg_mma3_mn_steps<kTileK / 16>(d, sa, sa + S::kA, sb, sb + S::kB, GROUP, kt != 0);
+        wg_mma_mn_steps<kTileK / 16, NP>(d, sa, sa + S::kA, sb, sb + S::kB, GROUP, kt != 0);
         wgmma_commit();
     }
     wgmma_wait<0>();
@@ -354,7 +366,7 @@ struct WgMultiArgs {
     int Cin, Cout, ksize;
 };
 
-template <int BC, int STAGES>
+template <int BC, int STAGES, int NP>
 __global__ void __launch_bounds__(kTcThreads, 1)
 wgrad_tc2_multi_kernel(const __grid_constant__ WgMaps maps, const __grid_constant__ WgMultiArgs a, const int chunks_per_split,
                        const int ctiles) {
@@ -400,13 +412,13 @@ wgrad_tc2_multi_kernel(const __grid_constant__ WgMaps maps, const __grid_constan
                 const int by = ch % g.nby;
                 const int bb = ch / g.nby;
                 const int x0 = bx * g.Wb, y0 = by * g.Hb, b0 = bb * g.Bb;
-                const uint32_t bytes = (uint32_t)(2 * (kTileM / 64 + BC / 64) * g.kstage * 128);
+                const uint32_t bytes = (uint32_t)((NP == 3 ? 2 : 1) * (kTileM / 64 + BC / 64) * g.kstage * 128);
                 mbar_wait(&empty_bar[s], ph ^ 1);
                 mbar_arrive_expect_tx(&full_bar[s], bytes);
                 uint8_t* a_hi = smem + s * S::kStage;
                 uint8_t* b_hi = a_hi + 2 * S::kA;
 #pragma unroll
-                for (int pl = 0; pl < 2; ++pl) {
+                for (int pl = 0; pl < (NP == 3 ? 2 : 1); ++pl) {
 #pragma unroll
                     for (int q = 0; q < kTileM / 64; ++q)
                         tma_load_5d(a_hi + pl * S::kA + q * GROUP, &maps.dy[l], &full_bar[s], n0 + q * 64, x0, y0, b0, pl);
@@ -430,7 +442,7 @@ wgrad_tc2_multi_kernel(const __grid_constant__ WgMaps maps, const __grid_constan
                     mbar_wait(&full_bar[s], ph);
                     const uint32_t sa = smem_u32(smem + s * S::kStage) + wg * GROUP;
                     const uint32_t sb = smem_u32(smem + s * S::kStage) + 2 * S::kA;
-                    wg_mma3_mn_steps<ksteps>(d, sa, sa + S::kA, sb, sb + S::kB, GROUP, kt != 0);
+                    wg_mma_mn_steps<ksteps, NP>(d, sa, sa + S::kA, sb, sb + S::kB, GROUP, kt != 0);
                     wgmma_commit();
                     wgmma_wait<1>();
                     if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % STAGES]);
@@ -525,14 +537,19 @@ int conv_tc_launch(const effdet_conv_args* levels, int nlevels, cudaStream_t st)
     ma.nlevels = nlevels;
     int tiles = 0;
     for (int l = 0; l < nlevels; ++l) {
-        ma.lv[l] = levels[l];
+        ma.lv[l].set(levels[l]);
         ma.tile_begin[l] = tiles;
         tiles += cdiv((long long)levels[l].B * levels[l].H * levels[l].W, kTileM);
     }
     for (int l = nlevels; l <= kMaxLevels; ++l) ma.tile_begin[l] = tiles;
     dim3 grid(tiles, cdiv(a->Cout, BN));
-    if (BN == 64) return launch_smem("conv_tc_kernel", conv_tc_kernel<64, 4>, grid, kTcThreads, FwdSmem<64, 4>::kBytes, st, map, ma, kblocks);
-    return launch_smem("conv_tc_kernel", conv_tc_kernel<128, 3>, grid, kTcThreads, FwdSmem<128, 3>::kBytes, st, map, ma, kblocks);
+    if (a->tc_single) {
+        if (BN == 64)
+            return launch_smem("conv_tc_kernel", conv_tc_kernel<64, 4, 1>, grid, kTcThreads, FwdSmem<64, 4>::kBytes, st, map, ma, kblocks);
+        return launch_smem("conv_tc_kernel", conv_tc_kernel<128, 3, 1>, grid, kTcThreads, FwdSmem<128, 3>::kBytes, st, map, ma, kblocks);
+    }
+    if (BN == 64) return launch_smem("conv_tc_kernel", conv_tc_kernel<64, 4, 3>, grid, kTcThreads, FwdSmem<64, 4>::kBytes, st, map, ma, kblocks);
+    return launch_smem("conv_tc_kernel", conv_tc_kernel<128, 3, 3>, grid, kTcThreads, FwdSmem<128, 3>::kBytes, st, map, ma, kblocks);
 }
 
 bool wgrad_tc_eligible(const effdet_wgrad_args* a) {
@@ -628,10 +645,17 @@ static int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaSt
     int cps = cdiv(chunks, splits);
     splits = cdiv(chunks, cps);
     dim3 grid(ctiles * ntiles, taps, splits);
-    if (BC == 256)
-        return launch_smem("wgrad_tc2_multi_kernel", wgrad_tc2_multi_kernel<256, 2>, grid, kTcThreads, WgSmem<256, 2>::kBytes, st,
+    if (a0->tc_single) {
+        if (BC == 256)
+            return launch_smem("wgrad_tc2_multi_kernel", wgrad_tc2_multi_kernel<256, 2, 1>, grid, kTcThreads, WgSmem<256, 2>::kBytes,
+                               st, maps, ma, cps, ctiles);
+        return launch_smem("wgrad_tc2_multi_kernel", wgrad_tc2_multi_kernel<64, 4, 1>, grid, kTcThreads, WgSmem<64, 4>::kBytes, st,
                            maps, ma, cps, ctiles);
-    return launch_smem("wgrad_tc2_multi_kernel", wgrad_tc2_multi_kernel<64, 4>, grid, kTcThreads, WgSmem<64, 4>::kBytes, st, maps,
+    }
+    if (BC == 256)
+        return launch_smem("wgrad_tc2_multi_kernel", wgrad_tc2_multi_kernel<256, 2, 3>, grid, kTcThreads, WgSmem<256, 2>::kBytes, st,
+                           maps, ma, cps, ctiles);
+    return launch_smem("wgrad_tc2_multi_kernel", wgrad_tc2_multi_kernel<64, 4, 3>, grid, kTcThreads, WgSmem<64, 4>::kBytes, st, maps,
                        ma, cps, ctiles);
 }
 
@@ -651,10 +675,19 @@ int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st, bool* dbias_don
     int cps = cdiv(nchunks, splits);
     splits = cdiv(nchunks, cps);
     dim3 grid(ctiles * ntiles, taps, splits);
-    if (BC == 256)
-        return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<256, 2>, grid, kTcProducers, WgSmem<256, 2>::kBytes, st, *a, M, HW, cps,
+    WgradPrefix pa;
+    pa.set(*a);
+    if (a->tc_single) {
+        if (BC == 256)
+            return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<256, 2, 1>, grid, kTcProducers, WgSmem<256, 2>::kBytes, st, pa, M, HW,
+                               cps, ctiles);
+        return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<64, 4, 1>, grid, kTcProducers, WgSmem<64, 4>::kBytes, st, pa, M, HW, cps,
                            ctiles);
-    return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<64, 4>, grid, kTcProducers, WgSmem<64, 4>::kBytes, st, *a, M, HW, cps, ctiles);
+    }
+    if (BC == 256)
+        return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<256, 2, 3>, grid, kTcProducers, WgSmem<256, 2>::kBytes, st, pa, M, HW, cps,
+                           ctiles);
+    return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<64, 4, 3>, grid, kTcProducers, WgSmem<64, 4>::kBytes, st, pa, M, HW, cps, ctiles);
 }
 
 }  // namespace effdet
@@ -674,6 +707,9 @@ extern "C" int effdet_conv2d_wgrad_multi(const effdet_wgrad_args* levels, int nl
         const effdet_wgrad_args* a = &levels[l];
         EFFDET_REQUIRE((a->x || a->x_planes) && (a->dy || a->dy_planes) && a->dw, "conv2d_wgrad_multi: null tensor");
         EFFDET_REQUIRE(!(a->dy_planes && a->dbias), "conv2d_wgrad_multi: dy_planes excludes dbias (the producer supplies the column sums)");
+        EFFDET_REQUIRE(a->tc_single == levels[0].tc_single, "conv2d_wgrad_multi: levels disagree on tc_single");
+        EFFDET_REQUIRE(!a->tc_single || (a->precision == 1 && a->ksize == 3),
+                       "conv2d_wgrad_multi: tc_single needs precision 1 and a 3x3 convolution");
         same = same && a->dw == levels[0].dw && a->dbias == levels[0].dbias && a->Cin == levels[0].Cin &&
                a->Cout == levels[0].Cout && a->ksize == levels[0].ksize && a->precision == 1 && wgrad_tc_eligible(a);
     }
@@ -700,6 +736,8 @@ extern "C" int effdet_conv2d_multi(const effdet_conv_args* levels, int nlevels, 
                            a->act == levels[0].act && a->w == levels[0].w && a->w_tc == levels[0].w_tc &&
                            a->bias == levels[0].bias,
                        "conv2d_multi: all levels must share weights, bias, channels and activation");
+        EFFDET_REQUIRE(a->tc_single == levels[0].tc_single, "conv2d_multi: levels disagree on tc_single");
+        EFFDET_REQUIRE(!a->tc_single || (a->w_tc && a->ksize == 3), "conv2d_multi: tc_single needs w_tc and a 3x3 convolution");
         tc = tc && conv_tc_eligible(a) && (long long)a->B * a->H * a->W < (1ll << 31);
         EFFDET_REQUIRE(aligned16(a->x) && aligned16(a->y) && aligned16(a->residual) && aligned16(a->mask_src) &&
                            a->x_bstride % 4 == 0 && a->y_bstride % 4 == 0 && a->r_bstride % 4 == 0 && a->m_bstride % 4 == 0,

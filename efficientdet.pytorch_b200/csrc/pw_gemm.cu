@@ -220,7 +220,7 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {                  // K is zero-padded to 64 per block (weights and A planes)
-                    wg_mma3<NB, 0>(d, a_hi + k * 32, a_lo + k * 32, b_hi + k * 32, b_lo + k * 32, 16, 1024, (kb | k) != 0);
+                    wg_mma<NB, 0, 3>(d, a_hi + k * 32, a_lo + k * 32, b_hi + k * 32, b_lo + k * 32, 16, 1024, (kb | k) != 0);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();                               // the previous k-block's operands are no longer read

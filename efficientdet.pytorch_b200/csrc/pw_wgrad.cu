@@ -205,7 +205,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) pw_wgrad_kernel(const __grid_co
                 mbar_wait(&full_bar[s], ph);
                 const uint32_t a_hi = smem_u32(smem + (size_t)s * P.stage_bytes) + a_off;
                 const uint32_t b_hi = smem_u32(smem + (size_t)s * P.stage_bytes) + 2 * P.a_plane;
-                wg_mma3_mn_steps<ksteps>(d, a_hi, a_hi + P.a_plane, b_hi, b_hi + P.b_plane, group, kt != 0);
+                wg_mma_mn_steps<ksteps, 3>(d,a_hi, a_hi + P.a_plane, b_hi, b_hi + P.b_plane, group, kt != 0);
                 wgmma_commit();
                 wgmma_wait<1>();                               // the previous stage is no longer read
                 if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % P.NS]);

@@ -5,6 +5,7 @@
 
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <stddef.h>
 #include <type_traits>
 
 namespace effdet {
@@ -124,29 +125,36 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[4][32], uint64_t desc_a, u
 }
 #undef EFFDET_WG_D32
 #undef EFFDET_WG_D8
-// One K16 step of the split-precision product over all NB*64 columns: lo*hi + hi*lo + hi*hi (x ~= hi + lo), one
-// full-width wgmma per product, so every accumulator element sums the three products in that order.
+// One K16 step over all NB*64 columns with P bf16 products per multiply-add (P = 3 is the default, bf16x3 precision;
+// P = 1 is EFFDET_B200_PRECISION=bf16 on the dense 3x3 convs), one full-width wgmma per product:
+//   P = 3  split precision, lo*hi + hi*lo + hi*hi (x ~= hi + lo), every accumulator element sums them in that order
+//   P = 1  single pass, hi*hi only (the lo planes are not read)
 // a_*: this warpgroup's 64-row slice.  The descriptor locates the B operand's 64-column blocks: 8 * sbo bytes apart
 // for K-major operands (64 rows of 128 bytes), lbo bytes apart for MN-major ones.
-template <int NB, int MN>
-__device__ __forceinline__ void wg_mma3(float (&d)[NB][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
-                                        uint32_t lbo, uint32_t sbo, uint32_t accumulate) {
-    const uint64_t dah = gmma_desc(a_hi, lbo, sbo), dal = gmma_desc(a_lo, lbo, sbo);
-    const uint64_t dbh = gmma_desc(b_hi, lbo, sbo), dbl = gmma_desc(b_lo, lbo, sbo);
-    wgmma_bf16<MN>(d, dal, dbh, accumulate);
-    wgmma_bf16<MN>(d, dah, dbl, 1);
-    wgmma_bf16<MN>(d, dah, dbh, 1);
+template <int NB, int MN, int P>
+__device__ __forceinline__ void wg_mma(float (&d)[NB][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                       uint32_t lbo, uint32_t sbo, uint32_t accumulate) {
+    static_assert(P == 1 || P == 3, "one or three bf16 products per multiply-add");
+    if constexpr (P == 3) {
+        const uint64_t dah = gmma_desc(a_hi, lbo, sbo), dal = gmma_desc(a_lo, lbo, sbo);
+        const uint64_t dbh = gmma_desc(b_hi, lbo, sbo), dbl = gmma_desc(b_lo, lbo, sbo);
+        wgmma_bf16<MN>(d, dal, dbh, accumulate);
+        wgmma_bf16<MN>(d, dah, dbl, 1);
+        wgmma_bf16<MN>(d, dah, dbh, 1);
+    } else {
+        wgmma_bf16<MN>(d, gmma_desc(a_hi, lbo, sbo), gmma_desc(b_hi, lbo, sbo), accumulate);
+    }
 }
 // KS K16 steps of one stage of MN-major operands (the weight gradients: GEMM-K = pixel rows, a K16 step is two 8-row
-// groups, SBO = 1024 bytes apart; 64-channel groups `group` bytes apart), fully unrolled.
-template <int KS, int NB>
-__device__ __forceinline__ void wg_mma3_mn_steps(float (&d)[NB][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
-                                                 uint32_t group, uint32_t accumulate) {
+// groups, SBO = 1024 bytes apart; 64-channel groups `group` bytes apart), fully unrolled, P products per multiply-add.
+template <int KS, int P, int NB>
+__device__ __forceinline__ void wg_mma_mn_steps(float (&d)[NB][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                                uint32_t group, uint32_t accumulate) {
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < KS; ++k) {
         const uint32_t ko = k * 2 * 1024;
-        wg_mma3<NB, 1>(d, a_hi + ko, a_lo + ko, b_hi + ko, b_lo + ko, group, 1024, accumulate | k);
+        wg_mma<NB, 1, P>(d, a_hi + ko, a_lo + ko, b_hi + ko, b_lo + ko, group, 1024, accumulate | k);
     }
 }
 // Calls f(std::integral_constant<int, n>()) for the one count among KS... that equals n: a warp-uniform branch into one
@@ -205,6 +213,13 @@ __device__ __forceinline__ void split8(const float4 a, const float4 b, uint4& hi
     hi = make_uint4(h[0], h[1], h[2], h[3]);
     lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
+// the "hi" half of split8 alone (round to nearest bf16), for the single-pass kernels
+__device__ __forceinline__ uint4 hi8(const float4 a, const float4 b) {
+    const __nv_bfloat162 h0 = __floats2bfloat162_rn(a.x, a.y), h1 = __floats2bfloat162_rn(a.z, a.w);
+    const __nv_bfloat162 h2 = __floats2bfloat162_rn(b.x, b.y), h3 = __floats2bfloat162_rn(b.z, b.w);
+    return make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1),
+                      *reinterpret_cast<const uint32_t*>(&h2), *reinterpret_cast<const uint32_t*>(&h3));
+}
 
 
 // ---- additions for the persistent pointwise GEMM (pw_gemm.cu) -------------------------------------------------------
@@ -250,6 +265,17 @@ int launch_smem(const char* name, void (*kernel)(P...), dim3 grid, int threads, 
     kernel<<<grid, threads, smem, st>>>(args...);
     return launch_status(name);
 }
+
+// A kernel's copy of an ABI argument struct: its bytes up to the trailing tc_single, which selects the kernel instance
+// instead of being read on the device.  So the parameter blocks keep the layout they had before the field was appended.
+template <class T, size_t N>
+struct alignas(8) ArgsPrefix {
+    unsigned char raw[N];
+    __host__ __device__ const T& get() const { return *reinterpret_cast<const T*>(raw); }
+    void set(const T& a) { memcpy(raw, &a, N); }
+};
+using ConvLevel = ArgsPrefix<effdet_conv_args, offsetof(effdet_conv_args, tc_single)>;
+using WgradPrefix = ArgsPrefix<effdet_wgrad_args, offsetof(effdet_wgrad_args, tc_single)>;
 
 // Pixel boxes of the TMA-fed kernels: a [B,H,W,*] map is tiled into boxes of Wb x Hb x Bb = kstage pixels (16..64, a
 // multiple of 16) that one tensor-map load turns into kstage consecutive 128-byte rows of shared memory (conv_tc.cu)

@@ -76,14 +76,14 @@ class ConvArgs(ctypes.Structure):
                 ('bias', _P), ('scale', _P), ('shift', _P), ('a_scale', _P), ('row_scale', _P),
                 ('residual', _P), ('r_bstride', _I64), ('mask_src', _P), ('m_bstride', _I64),
                 ('B', _I32), ('H', _I32), ('W', _I32), ('Cin', _I32), ('Cout', _I32), ('ksize', _I32), ('act', _I32),
-                ('w_tc', _P), ('in_scale', _P), ('in_shift', _P), ('x_planes', _P)]
+                ('w_tc', _P), ('in_scale', _P), ('in_shift', _P), ('x_planes', _P), ('tc_single', _I32)]
 
 
 class WgradArgs(ctypes.Structure):
     _fields_ = [('x', _P), ('x_bstride', _I64), ('dy', _P), ('dy_bstride', _I64), ('dw', _P), ('dbias', _P),
                 ('a_scale', _P), ('B', _I32), ('H', _I32), ('W', _I32), ('Cin', _I32), ('Cout', _I32), ('ksize', _I32),
                 ('precision', _I32), ('ws_x', _P), ('ws_dy', _P), ('in_scale', _P), ('in_shift', _P), ('dy_planes', _P),
-                ('x_planes', _P)]
+                ('x_planes', _P), ('tc_single', _I32)]
 
 
 class BnActBwdArgs(ctypes.Structure):
@@ -95,7 +95,8 @@ class BnActBwdArgs(ctypes.Structure):
 class ConvPlanesArgs(ctypes.Structure):
     _fields_ = [('x_planes', _P), ('w_tc', _P), ('bias', _P), ('y', _P), ('y_bstride', _I64), ('y_planes', _P),
                 ('mask_planes', _P), ('residual', _P), ('r_bstride', _I64), ('colsum', _P),
-                ('B', _I32), ('H', _I32), ('W', _I32), ('Cin', _I32), ('Cout', _I32), ('ksize', _I32), ('act', _I32)]
+                ('B', _I32), ('H', _I32), ('W', _I32), ('Cin', _I32), ('Cout', _I32), ('ksize', _I32), ('act', _I32),
+                ('tc_single', _I32)]
 
 
 class DwFwdArgs(ctypes.Structure):

@@ -139,12 +139,21 @@ def pack_conv(w):
 # Precision of the dense 1x1 / 3x3 convolutions of neck and head (95 % of the FLOPs):
 #   'bf16x3' (default): wgmma tensor cores, operands split into bf16 hi+lo, three MMAs per product
 #                       (~2^-16 relative per product, fp32 accumulation)
+#   'bf16'            : the same routing, but the dense 3x3 convs (BiFPN nodes, head towers, class / box convs; forward,
+#                       data and weight gradient) take one MMA per product: bf16-rounded operands, fp32 accumulation.
+#                       The 1x1 convs stay on bf16x3 (they are HBM-bound, a single pass would buy no time)
 #   'fp32'            : exact fp32 FMA on the CUDA cores
 PRECISION = os.environ.get('EFFDET_B200_PRECISION', 'bf16x3')
 
 
 def tc_enabled():
-    return PRECISION == 'bf16x3'
+    """route the dense convs to the tensor cores (bf16x3 or bf16 mode)"""
+    return PRECISION in ('bf16x3', 'bf16')
+
+
+def tc_single(k):
+    """1 when a k x k tensor-core conv takes one bf16 product per multiply-add (bf16 mode, 3x3 only), else 0"""
+    return 1 if PRECISION == 'bf16' and k == 3 else 0
 
 
 def pack_conv_tc(w):
@@ -203,7 +212,7 @@ def conv2d_raw(dev_t, x_ptr, x_bs, wf, y_ptr, y_bs, B, H, W, Cin, Cout, k, z_ptr
                    N.f32(scale, 'scale'), N.f32(shift, 'shift'), N.f32(a_scale, 'a_scale'),
                    N.f32(row_scale, 'row_scale'), res_ptr, res_bs, mask_ptr, mask_bs, B, H, W, Cin, Cout, k, act,
                    w_tc.data_ptr() if w_tc is not None else None, N.f32(in_scale, 'in_scale'),
-                   N.f32(in_shift, 'in_shift'), N.ptr(x_planes))
+                   N.f32(in_shift, 'in_shift'), N.ptr(x_planes), tc_single(k) if w_tc is not None else 0)
     N.call('effdet_conv2d', dev_t, a)
 
 
@@ -244,10 +253,11 @@ def conv2d_multi_raw(dev_t, levels, wf, Cin, Cout, k, bias=None, act=ACT_NONE, w
     arr = (N.ConvArgs * nl)()
     wfp, bp = N.f32(wf, 'packed weight'), N.f32(bias, 'bias')
     tcp = w_tc.data_ptr() if w_tc is not None else None
+    single = tc_single(k) if w_tc is not None else 0
     for i, lv in enumerate(levels):
         arr[i] = N.ConvArgs(lv['x_ptr'], lv['x_bs'], wfp, lv['y_ptr'], lv['y_bs'], None, bp, None, None, None, None,
                             lv.get('res_ptr'), lv.get('res_bs', 0), lv.get('mask_ptr'), lv.get('mask_bs', 0),
-                            lv['B'], lv['H'], lv['W'], Cin, Cout, k, act, tcp)
+                            lv['B'], lv['H'], lv['W'], Cin, Cout, k, act, tcp, tc_single=single)
     N.call('effdet_conv2d_multi', dev_t, arr, nl)
 
 
@@ -279,7 +289,7 @@ def conv_wgrad_raw(dev_t, x_ptr, x_bs, dy_ptr, dy_bs, dw, dbias, B, H, W, Cin, C
     a = N.WgradArgs(x_ptr, x_bs, dy_ptr, dy_bs, N.f32(dw, 'dw'), N.f32(dbias, 'dbias'), N.f32(a_scale, 'a_scale'),
                     B, H, W, Cin, Cout, k, 1 if tc else 0, ws_x.data_ptr() if ws_x is not None else None,
                     ws_dy.data_ptr() if ws_dy is not None else None, N.f32(in_scale, 'in_scale'),
-                    N.f32(in_shift, 'in_shift'), N.ptr(dy_planes))
+                    N.f32(in_shift, 'in_shift'), N.ptr(dy_planes), None, tc_single(k) if tc else 0)
     N.call('effdet_conv2d_wgrad', dev_t, a)
 
 
@@ -305,7 +315,8 @@ def conv_wgrad_multi(dev_t, levels, dw, dbias, Cin, Cout, k, tc=False):
             keep += [ws_x, ws_dy]
         arr[i] = N.WgradArgs(lv['x_ptr'], lv['x_bs'], lv['dy_ptr'], lv['dy_bs'], N.f32(dw, 'dw'), N.f32(dbias, 'dbias'),
                              None, lv['B'], lv['H'], lv['W'], Cin, Cout, k, 1 if tc else 0,
-                             ws_x.data_ptr() if ws_x is not None else None, ws_dy.data_ptr() if ws_dy is not None else None)
+                             ws_x.data_ptr() if ws_x is not None else None, ws_dy.data_ptr() if ws_dy is not None else None,
+                             tc_single=tc_single(k) if tc else 0)
     N.call('effdet_conv2d_wgrad_multi', dev_t, arr, nl)
 
 
@@ -820,7 +831,7 @@ def conv_planes_multi(dev_t, levels, w_tc, Cin, Cout, k, bias=None, act=ACT_NONE
     for i, lv in enumerate(levels):
         arr[i] = N.ConvPlanesArgs(N.ptr(lv['x']), w_tc.data_ptr(), N.f32(bias, 'bias'), lv.get('y_ptr'), lv.get('y_bs', 0),
                                   N.ptr(lv.get('y_planes')), N.ptr(lv.get('mask')), lv.get('res_ptr'), lv.get('res_bs', 0),
-                                  N.f32(colsum, 'colsum'), lv['B'], lv['H'], lv['W'], Cin, Cout, k, act)
+                                  N.f32(colsum, 'colsum'), lv['B'], lv['H'], lv['W'], Cin, Cout, k, act, tc_single(k))
     px = sum(lv['B'] * lv['H'] * lv['W'] for lv in levels)
     N.call('effdet_conv_planes_multi', dev_t, arr, nl, flops=2.0 * px * k * k * Cin * Cout,
            nbytes=4.0 * (px * (Cin + Cout) + k * k * Cin * Cout))
@@ -833,7 +844,7 @@ def wgrad_planes_multi(dev_t, levels, dw, Cin, Cout, k):
     arr = (N.WgradArgs * nl)()
     for i, lv in enumerate(levels):
         arr[i] = N.WgradArgs(None, 0, None, 0, N.f32(dw, 'dw'), None, None, lv['B'], lv['H'], lv['W'], Cin, Cout, k, 1, None,
-                             None, None, None, N.ptr(lv['dy']), N.ptr(lv['x']))
+                             None, None, None, N.ptr(lv['dy']), N.ptr(lv['x']), tc_single(k))
     N.call('effdet_conv2d_wgrad_multi', dev_t, arr, nl)
 
 

@@ -70,7 +70,7 @@ typedef struct {
     int32_t B, H, W, Cin, Cout, ksize, act;
     const void* w_tc;      /* optional bf16 hi/lo planes from effdet_pack_conv_weight_tc: when set (and the
                               epilogue needs only bias/act/residual/mask) the layer runs on the wgmma
-                              tensor cores as a bf16x3 split-precision implicit GEMM (~2^-16 per product) */
+                              tensor cores as a bf16x3 split-precision implicit GEMM (~2^-16 per product; see tc_single) */
     const float* in_scale; const float* in_shift; /* [Cin] or both NULL: the input is a RAW conv output and the
                               operand is swish(x*in_scale+in_shift) (eval-BN + swish applied while the tile is
                               staged, so the activated tensor never exists in HBM: MemoryEfficientSwish keeps
@@ -78,6 +78,10 @@ typedef struct {
     const void* x_planes;  /* optional (1x1 convs, tensor-core path): the input PRE-SPLIT into bf16 planes
                               [2][B*H*W][Cin] (plane 0 = hi, plane 1 = lo, x ~= hi + lo; Cin % 8 == 0), as written by
                               effdet_dwconv_bwd_fused; x may then be NULL */
+    int32_t tc_single;     /* 1: when this call runs on the tensor cores, one bf16 product per multiply-add (hi(x)*hi(w),
+                              fp32 accumulation) instead of bf16x3; 3x3 convolutions only (ksize 1 -> EFFDET_ERR_ARG).
+                              0 keeps the bf16x3 split precision. Needs w_tc (else EFFDET_ERR_ARG); every level of a
+                              multi-level call must pass the same value */
 } effdet_conv_args;
 int effdet_conv2d(const effdet_conv_args* a, int device, effdet_stream_t stream);
 /* The same convolution (shared w / w_tc / bias / act, channels, ksize) applied to `nlevels` (<= 8) feature maps of
@@ -106,6 +110,10 @@ typedef struct {
                               by effdet_dwconv_bwd_fused / effdet_conv_planes_multi: no split pass over dy, ws_dy unused,
                               dy may be NULL (dbias must be NULL) */
     const void* x_planes;  /* optional, likewise for x ([2][B*H*W][pitch(Cin)]; no a_scale / in_scale): ws_x unused */
+    int32_t tc_single;     /* 1: when this call runs on the tensor cores, one bf16 product per multiply-add (hi(x)*hi(w),
+                              fp32 accumulation) instead of bf16x3; 3x3 convolutions only (ksize 1 -> EFFDET_ERR_ARG).
+                              0 keeps the bf16x3 split precision. Needs precision 1 (else EFFDET_ERR_ARG); every
+                              level of a multi-level call must pass the same value */
 } effdet_wgrad_args;
 int effdet_conv2d_wgrad(const effdet_wgrad_args* a, int device, effdet_stream_t stream);
 /* Weight gradient of one shared-weight layer accumulated over `nlevels` feature maps in one launch (all levels
@@ -133,6 +141,8 @@ typedef struct {
     const float* residual; int64_t r_bstride;   /* fp32 [B][H*W][Cout] added before the mask, or NULL */
     float* colsum;                              /* [Cout] += or NULL */
     int32_t B, H, W, Cin, Cout, ksize, act;
+    int32_t tc_single;                          /* 1: one bf16 product per multiply-add (hi planes only), as in
+                                                   effdet_conv_args; 3x3 only, the same on every level */
 } effdet_conv_planes_args;
 int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, int nlevels, int device, effdet_stream_t stream);
 /* fp32 [B][HW][C] (image stride x_bstride) -> planes [2][B*HW][pitch(C)]; with prob != NULL the value is first

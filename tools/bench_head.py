@@ -6,9 +6,11 @@ a 256->256 tower layer and the 256->720 class conv (9 anchors x 80 classes), eac
   wgrad  wgrad_planes_multi from the input and gradient planes
 Times are CUDA events around `iters` back-to-back launches; TFLOP/s are algorithmic (2 * pixels * 9 * Cin * Cout per
 launch; the tensor cores execute three bf16 products for each).  Every result is also reduced to checksums so that two
-builds can be compared.
-usage: python tools/bench_head.py [B] [size] [iters]"""
+builds can be compared.  mode (default bf16x3) selects the precision: bf16 runs the single-pass instances (one bf16
+product per multiply-add, the lo planes are not read).
+usage: python tools/bench_head.py [B] [size] [iters] [bf16x3|bf16]"""
 import os
+import subprocess
 import sys
 
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -17,7 +19,10 @@ import torch                      # noqa: E402
 from models import _native as N   # noqa: E402
 from models import _ops as ops    # noqa: E402
 
-B, size, iters = [int(v) for v in (sys.argv[1:4] + ['32', '512', '20'][len(sys.argv) - 1:])]
+B, size, iters = [int(v) for v in (sys.argv[1:4] + ['32', '512', '20'][len(sys.argv) - 1:])[:3]]
+mode = sys.argv[4] if len(sys.argv) > 4 else 'bf16x3'
+assert mode in ('bf16x3', 'bf16'), mode
+ops.PRECISION = mode
 dev = torch.device('cuda:0')
 g = torch.Generator(device=dev).manual_seed(0)
 sides = [size >> s for s in (3, 4, 5, 6, 7)]                  # P3..P7
@@ -100,7 +105,9 @@ def timed(fn):
     return e0.elapsed_time(e1) / iters
 
 
-print('levels', sides, 'B', B, 'pixels', px, 'iters', iters, 'device', torch.cuda.get_device_name(dev))
+card = subprocess.run(['nvidia-smi', '-i', str(dev.index or 0), '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                      capture_output=True, text=True).stdout.strip()
+print('levels', sides, 'B', B, 'pixels', px, 'iters', iters, 'mode', mode, 'card', card)
 for Cin, Cout, act in ((256, 256, N.ACT_RELU), (256, 720, N.ACT_SIGMOID)):
     fns, checksum = shape(Cin, Cout, act)
     flops = 2.0 * px * 9 * Cin * Cout
