@@ -11,13 +11,15 @@
 // Wb x Hb x Bb pixels delivers, for one tap, 64 channels of 16..64 pixels as consecutive 128-byte rows in the canonical
 // K-major SWIZZLE_128B layout; the tap shift is a coordinate offset and the hardware's out-of-bounds zero fill is the
 // convolution's zero padding.  The kernel is a warp-specialised Hopper GEMM:
-//   warp 8      TMA producer (activation boxes hi/lo + weight tile hi/lo -> mbarrier complete_tx), ring of stages that
-//               runs ahead into the next unit while the consumers are in their epilogue
-//   warps 0-7   two consumer warpgroups, one per 64-row half of the tile: 3 wgmma per K16 (lo*hi, hi*lo, hi*hi) with the
-//               accumulator in registers (single-pass instance, NP = 1: hi*hi only, and the producer loads no lo plane), then the epilogue: bias / ReLU / sigmoid / ReLU-mask / residual -> bf16 hi/lo
-//               planes (the next layer's operand) and / or fp32 (head outputs, data gradient w.r.t. the BiFPN features);
-//               optional per-channel column sums of what was stored (= the bias gradient of the producing layer)
-//               reduced by warp shuffles, one atomic per column per warp
+//   warp 8      TMA producer (activation boxes hi/lo + weight tile hi/lo -> mbarrier complete_tx), ring of stages
+//               filled in unit order
+//   warps 0-7   two consumer warpgroups in ping-pong: the CTA's units alternate between them, and each owns a whole
+//               128-row tile (two 64-row accumulator sets): 3 wgmma per K16 and row half (lo*hi, hi*lo, hi*hi) with the
+//               accumulator in registers (single-pass instance, NP = 1: hi*hi only, and the producer loads no lo plane),
+//               then the epilogue: bias / ReLU / sigmoid / ReLU-mask / residual -> bf16 hi/lo planes (the next layer's
+//               operand) and / or fp32 (head outputs, data gradient w.r.t. the BiFPN features); optional per-channel
+//               column sums of what was stored (= the bias gradient of the producing layer) reduced by warp shuffles,
+//               one atomic per column per warp.  One warpgroup's epilogue runs under the other's MMAs.
 // persistent over (pixel tile, channel tile) units of all pyramid levels that share the weights.
 #include "tc_ptx.cuh"
 
@@ -26,16 +28,22 @@
 namespace effdet {
 
 constexpr int kPlMaxLevels = 8;
-constexpr int kPlThreads = 288;
+// two consumer warpgroups and a producer warpgroup: ptxas budgets 168 registers per thread for 384 threads, and
+// setmaxnreg moves the producer's share to the consumers (128 x 40 + 256 x 232 = 384 x 168)
+constexpr int kPlThreads = 384;
+constexpr int kPlProducerRegs = 40, kPlConsumerRegs = 232;
 constexpr int kPlA = 128 * 128;            // one plane of the activation tile: 128 pixel rows x 64 channels (bf16)
-// BN = output channels per tile (accumulator: BN / 2 registers per consumer thread); the ring depth is what fits
+// BN = output channels per tile (accumulator: BN registers per consumer thread); the ring depth is what fits.  Behind
+// the ring: the two warpgroups' staging buffers (wg_rows_own), the mbarriers, the two warpgroups' bias buffers.
 template <int BN>
 struct PlCfg {
     static constexpr int kStages = BN == 128 ? 3 : 4;
     static constexpr int kB = BN * 128;    // one plane of the weight tile: BN output channels x 64 input channels
     static constexpr int kStage = 2 * kPlA + 2 * kB;
-    static constexpr int kSmem = kStages * kStage + kRowsBytes + 1024 + 256 + BN * 4;
+    static constexpr int kSmem = kStages * kStage + kRowsBytes + 1024 + 256 + 2 * BN * 4;
 };
+// named barriers of the consumer warpgroup g: 2 + g its staging buffer and bias buffer, 4 + g its turn to consume
+constexpr int kPlBarRows = 2, kPlBarTurn = 4;
 
 struct PlLevel {
     int B, H, W;
@@ -67,10 +75,10 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
     constexpr int kPlBN = BN, kPlStages = PlCfg<BN>::kStages, kPlB = PlCfg<BN>::kB, kPlStage = PlCfg<BN>::kStage;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1024-byte aligned AND still a shared-space pointer (LDS/STS, not generic LD/ST)
-    float* rows_buf = reinterpret_cast<float*>(smem + kPlStages * kPlStage);       // epilogue staging (wg_rows)
+    float* rows_buf = reinterpret_cast<float*>(smem + kPlStages * kPlStage);       // epilogue staging (wg_rows_own)
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kPlStages * kPlStage + kRowsBytes);
     uint64_t* empty_bar = full_bar + kPlStages;
-    float* chan = reinterpret_cast<float*>(smem + kPlStages * kPlStage + kRowsBytes + 256);   // bias of the current channel tile
+    float* chan_buf = reinterpret_cast<float*>(smem + kPlStages * kPlStage + kRowsBytes + 256);   // bias of the channel tile
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int taps = P.ksize * P.ksize, pad = P.ksize / 2;
@@ -78,7 +86,7 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
     if (threadIdx.x == 0) {
         for (int s = 0; s < kPlStages; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 8);     // one arrival per consumer warp
+            mbar_init(&empty_bar[s], 4);     // one arrival per warp of the warpgroup that consumes the stage
         }
         fence_barrier_init();
         tma_prefetch_desc(&wmap);
@@ -94,9 +102,10 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
         box0 = (mt - P.lv[l].tile_begin) * (128 / P.lv[l].g.kstage);
     };
 
-    if (warp == 8) {
-        // ---------------- TMA producer ------------------------------------------------------------------------------------
-        if (lane == 0) {
+    if (warp >= 8) {
+        // ---------------- TMA producer (one thread of warpgroup 2) ---------------------------------------------------------
+        setmaxnreg_dec<kPlProducerRegs>();
+        if (warp == 8 && lane == 0) {
             uint32_t it = 0;
             for (int unit = blockIdx.x; unit < P.total_tiles; unit += gridDim.x) {
                 int l, box0, n0;
@@ -129,136 +138,154 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
             }
         }
     } else {
-        // ---------------- consumer warpgroups: wgmma, then the epilogue ----------------------------------------------------
+        // ---------------- consumer warpgroups in ping-pong: wgmma of a whole tile, then its epilogue -----------------------
+        // The CTA's k-th unit belongs to warpgroup k & 1 and fills ring slots it = k * KT .. k * KT + KT - 1.  A
+        // warpgroup waits for its turn (barrier 4 + g) before it waits on the full barriers of its unit: then every
+        // slot before its own has been seen full, so no full barrier it polls is two phases behind the parity it
+        // asks for.  It hands the turn on as soon as its last stage has landed, so the other warpgroup's MMAs start
+        // while its own last ones and its epilogue run.
+        setmaxnreg_inc<kPlConsumerRegs>();
         constexpr int NB = kPlBN / 64;
-        const int g = warp >> 2;                                   // rows 64g .. 64g+63 of the tile
-        const int etid = threadIdx.x;
-        const int quarter = 2 * g + (warp & 1), half = (warp >> 1) & 1;
-        const int r = quarter * 32 + lane;                         // row of the tile owned by this thread
-        uint32_t it = 0;
+        const int g = warp >> 2;
+        const int half = (warp >> 1) & 1;                          // columns 32 * half .. + 31 of each 64x64 block
+        const int etid = threadIdx.x & 127;
+        float* rows = rows_buf + g * 32 * kRowsPitch;
+        float* chan = chan_buf + g * kPlBN;
+        const int nunits = (P.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
         int chan_n0 = -1;
-        for (int unit = blockIdx.x; unit < P.total_tiles; unit += gridDim.x) {
+        for (int k = g; k < nunits; k += 2) {
             int l, box0, n0;
-            decode(unit, l, box0, n0);
+            decode(blockIdx.x + k * gridDim.x, l, box0, n0);
             const PlLevel& L = P.lv[l];
-            float d[NB][32];
+            if (k > 0) named_bar_sync(kPlBarTurn + g, 256);
+            float d[2][NB][32];                                    // rows 0-63 and 64-127 of the tile
+            uint32_t it = (uint32_t)k * KT;
             for (int kt = 0; kt < KT; ++kt, ++it) {
                 const int s = it % kPlStages;
                 const uint32_t ph = (it / kPlStages) & 1;
                 mbar_wait(&full_bar[s], ph);
-                const uint32_t sa = smem_u32(smem + s * kPlStage) + g * 64 * 128;
-                const uint32_t sb = smem_u32(smem + s * kPlStage) + 2 * kPlA;
+                const uint32_t sa = smem_u32(smem + s * kPlStage);
+                const uint32_t sb = sa + 2 * kPlA;
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    wg_mma<NB, 0, NP>(d, sa + k * 32, sa + kPlA + k * 32, sb + k * 32, sb + kPlB + k * 32, 16, 1024, (kt | k) != 0);
+                for (int k16 = 0; k16 < 4; ++k16) {
+#pragma unroll
+                    for (int m = 0; m < 2; ++m)
+                        wg_mma<NB, 0, NP>(d[m], sa + m * 64 * 128 + k16 * 32, sa + kPlA + m * 64 * 128 + k16 * 32, sb + k16 * 32,
+                                          sb + kPlB + k16 * 32, 16, 1024, (kt | k16) != 0);
+                }
                 wgmma_commit();
                 wgmma_wait<1>();                                   // the previous stage is no longer read
                 if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kPlStages]);
             }
+            if (k + 1 < nunits) named_bar_arrive(kPlBarTurn + (g ^ 1), 256);
             wgmma_wait<0>();
             if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kPlStages]);
             if (n0 != chan_n0) {
-                named_bar_sync(1, 256);
-                for (int i = etid; i < kPlBN; i += 256) chan[i] = (n0 + i < P.Cout && P.bias) ? __ldg(P.bias + n0 + i) : 0.f;
-                named_bar_sync(1, 256);
+                named_bar_sync(kPlBarRows + g, 128);
+                for (int i = etid; i < kPlBN; i += 128) chan[i] = (n0 + i < P.Cout && P.bias) ? __ldg(P.bias + n0 + i) : 0.f;
+                named_bar_sync(kPlBarRows + g, 128);
                 chan_n0 = n0;
             }
-            // pixel of row r: box q of the tile, position i inside the box (x fastest, then y, then image)
-            const int ks = L.g.kstage;
-            const int q = r / ks, i = r - q * ks;
-            int ch = box0 + q;
-            bool row_ok = ch < L.nboxes;
-            const int bx = ch % L.g.nbx;
-            ch /= L.g.nbx;
-            const int by = ch % L.g.nby;
-            const int bb = ch / L.g.nby;
-            const int wh = L.g.Wb * L.g.Hb;
-            const int bi = i / wh, rem = i - bi * wh;
-            const int yy = rem / L.g.Wb, xx = rem - yy * L.g.Wb;
-            const int b = bb * L.g.Bb + bi, y = by * L.g.Hb + yy, x = bx * L.g.Wb + xx;
-            row_ok = row_ok && b < L.B;
-            const long long pixb = (long long)y * L.W + x;                     // pixel inside its image
-            const long long pix = (long long)b * L.H * L.W + pixb;             // pixel in the planes
             const long long plane = (long long)L.B * L.H * L.W * P.opitch;
             const int ncols = min(kPlBN, P.Cout - n0);
             const int nchunks = (ncols + 31) >> 5;
 #pragma unroll
-            for (int jb = 0; jb < NB; ++jb) {
-                float v[32];
-                wg_rows<2>(d[jb], rows_buf, g, v);
-                const int cc = 2 * jb + half;
-                if (cc >= nchunks) continue;
-                const int nb = n0 + cc * 32;                        // first channel of the chunk
+            for (int m = 0; m < 2; ++m) {
+                // pixel of row r: box q of the tile, position i inside the box (x fastest, then y, then image)
+                const int r = m * 64 + (warp & 1) * 32 + lane;         // row of the tile owned by this thread
+                const int ks = L.g.kstage;
+                const int q = r / ks, i = r - q * ks;
+                int ch = box0 + q;
+                bool row_ok = ch < L.nboxes;
+                const int bx = ch % L.g.nbx;
+                ch /= L.g.nbx;
+                const int by = ch % L.g.nby;
+                const int bb = ch / L.g.nby;
+                const int wh = L.g.Wb * L.g.Hb;
+                const int bi = i / wh, rem = i - bi * wh;
+                const int yy = rem / L.g.Wb, xx = rem - yy * L.g.Wb;
+                const int b = bb * L.g.Bb + bi, y = by * L.g.Hb + yy, x = bx * L.g.Wb + xx;
+                row_ok = row_ok && b < L.B;
+                const long long pixb = (long long)y * L.W + x;                     // pixel inside its image
+                const long long pix = (long long)b * L.H * L.W + pixb;             // pixel in the planes
 #pragma unroll
-                for (int k = 0; k < 32; ++k) {
-                    float t = v[k] + chan[cc * 32 + k];
-                    if (P.act == EFFDET_ACT_RELU) t = fmaxf(t, 0.f);
-                    else if (P.act == EFFDET_ACT_SIGMOID) t = sigmoidf_(t);
-                    v[k] = t;
-                }
-                if (row_ok && L.residual) {
+                for (int jb = 0; jb < NB; ++jb) {
+                    float v[32];
+                    wg_rows_own(d[m][jb], rows, kPlBarRows + g, v);
+                    const int cc = 2 * jb + half;
+                    if (cc >= nchunks) continue;
+                    const int nb = n0 + cc * 32;                        // first channel of the chunk
 #pragma unroll
-                    for (int k4 = 0; k4 < 8; ++k4) {
-                        if (nb + k4 * 4 >= P.Cout) break;
-                        const float4 rv = ldg4(L.residual + (long long)b * L.r_bstride + pixb * P.Cout + nb + k4 * 4);
-                        v[k4 * 4] += rv.x; v[k4 * 4 + 1] += rv.y; v[k4 * 4 + 2] += rv.z; v[k4 * 4 + 3] += rv.w;
+                    for (int k = 0; k < 32; ++k) {
+                        float t = v[k] + chan[cc * 32 + k];
+                        if (P.act == EFFDET_ACT_RELU) t = fmaxf(t, 0.f);
+                        else if (P.act == EFFDET_ACT_SIGMOID) t = sigmoidf_(t);
+                        v[k] = t;
                     }
-                }
-                if (row_ok && L.mask_planes) {                     // gradient passes where the forward activation was > 0
-                    const __nv_bfloat16* mh = L.mask_planes + pix * P.opitch + nb;
+                    if (row_ok && L.residual) {
 #pragma unroll
-                    for (int k8 = 0; k8 < 4; ++k8) {
-                        if (nb + k8 * 8 >= P.Cout) break;
-                        const uint4 hv = __ldg(reinterpret_cast<const uint4*>(mh + k8 * 8));
-                        const uint4 lv = __ldg(reinterpret_cast<const uint4*>(mh + plane + k8 * 8));
-                        const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) {
-                            const uint32_t hb = (hw[e >> 1] >> ((e & 1) * 16)) & 0xffffu, lb = (lw[e >> 1] >> ((e & 1) * 16)) & 0xffffu;
-                            // bf16 bits: positive and non-zero  <=>  sign clear and magnitude bits set
-                            const bool pos = (hb & 0x7fffu) ? !(hb & 0x8000u) : ((lb & 0x7fffu) && !(lb & 0x8000u));
-                            if (!pos) v[k8 * 8 + e] = 0.f;
+                        for (int k4 = 0; k4 < 8; ++k4) {
+                            if (nb + k4 * 4 >= P.Cout) break;
+                            const float4 rv = ldg4(L.residual + (long long)b * L.r_bstride + pixb * P.Cout + nb + k4 * 4);
+                            v[k4 * 4] += rv.x; v[k4 * 4 + 1] += rv.y; v[k4 * 4 + 2] += rv.z; v[k4 * 4 + 3] += rv.w;
                         }
                     }
-                }
-                if (!row_ok) {
+                    if (row_ok && L.mask_planes) {                     // gradient passes where the forward activation was > 0
+                        const __nv_bfloat16* mh = L.mask_planes + pix * P.opitch + nb;
 #pragma unroll
-                    for (int k = 0; k < 32; ++k) v[k] = 0.f;
-                }
-                if (row_ok && L.y) {
-                    float* yo = L.y + (long long)b * L.y_bstride + pixb * P.Cout + nb;
+                        for (int k8 = 0; k8 < 4; ++k8) {
+                            if (nb + k8 * 8 >= P.Cout) break;
+                            const uint4 hv = __ldg(reinterpret_cast<const uint4*>(mh + k8 * 8));
+                            const uint4 lv = __ldg(reinterpret_cast<const uint4*>(mh + plane + k8 * 8));
+                            const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
 #pragma unroll
-                    for (int k4 = 0; k4 < 8; ++k4) {
-                        if (nb + k4 * 4 >= P.Cout) break;
-                        st4(yo + k4 * 4, make_float4(v[k4 * 4], v[k4 * 4 + 1], v[k4 * 4 + 2], v[k4 * 4 + 3]));
-                    }
-                }
-                if (row_ok && L.y_planes) {
-                    __nv_bfloat16* ph = L.y_planes + pix * P.opitch + nb;
-#pragma unroll
-                    for (int k8 = 0; k8 < 4; ++k8) {
-                        if (nb + k8 * 8 >= P.Cout) break;
-                        uint4 hi, lo;
-                        split8(make_float4(v[k8 * 8], v[k8 * 8 + 1], v[k8 * 8 + 2], v[k8 * 8 + 3]),
-                               make_float4(v[k8 * 8 + 4], v[k8 * 8 + 5], v[k8 * 8 + 6], v[k8 * 8 + 7]), hi, lo);
-                        *reinterpret_cast<uint4*>(ph + k8 * 8) = hi;
-                        *reinterpret_cast<uint4*>(ph + plane + k8 * 8) = lo;
-                    }
-                }
-                if (P.colsum) {
-                    // warp transpose-reduce: afterwards v[0] of lane j is the sum over the warp's 32 rows of column j
-#pragma unroll
-                    for (int off = 16; off >= 1; off >>= 1) {
-                        const bool upper = (lane & off) != 0;
-#pragma unroll
-                        for (int k = 0; k < off; ++k) {
-                            const float send = upper ? v[k] : v[k + off];
-                            const float keep = upper ? v[k + off] : v[k];
-                            v[k] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+                            for (int e = 0; e < 8; ++e) {
+                                const uint32_t hb = (hw[e >> 1] >> ((e & 1) * 16)) & 0xffffu, lb = (lw[e >> 1] >> ((e & 1) * 16)) & 0xffffu;
+                                // bf16 bits: positive and non-zero  <=>  sign clear and magnitude bits set
+                                const bool pos = (hb & 0x7fffu) ? !(hb & 0x8000u) : ((lb & 0x7fffu) && !(lb & 0x8000u));
+                                if (!pos) v[k8 * 8 + e] = 0.f;
+                            }
                         }
                     }
-                    if (nb + lane < P.Cout) atomicAdd(P.colsum + nb + lane, v[0]);
+                    if (!row_ok) {
+#pragma unroll
+                        for (int k = 0; k < 32; ++k) v[k] = 0.f;
+                    }
+                    if (row_ok && L.y) {
+                        float* yo = L.y + (long long)b * L.y_bstride + pixb * P.Cout + nb;
+#pragma unroll
+                        for (int k4 = 0; k4 < 8; ++k4) {
+                            if (nb + k4 * 4 >= P.Cout) break;
+                            st4(yo + k4 * 4, make_float4(v[k4 * 4], v[k4 * 4 + 1], v[k4 * 4 + 2], v[k4 * 4 + 3]));
+                        }
+                    }
+                    if (row_ok && L.y_planes) {
+                        __nv_bfloat16* ph = L.y_planes + pix * P.opitch + nb;
+#pragma unroll
+                        for (int k8 = 0; k8 < 4; ++k8) {
+                            if (nb + k8 * 8 >= P.Cout) break;
+                            uint4 hi, lo;
+                            split8(make_float4(v[k8 * 8], v[k8 * 8 + 1], v[k8 * 8 + 2], v[k8 * 8 + 3]),
+                                   make_float4(v[k8 * 8 + 4], v[k8 * 8 + 5], v[k8 * 8 + 6], v[k8 * 8 + 7]), hi, lo);
+                            *reinterpret_cast<uint4*>(ph + k8 * 8) = hi;
+                            *reinterpret_cast<uint4*>(ph + plane + k8 * 8) = lo;
+                        }
+                    }
+                    if (P.colsum) {
+                        // warp transpose-reduce: afterwards v[0] of lane j is the sum over the warp's 32 rows of column j
+#pragma unroll
+                        for (int off = 16; off >= 1; off >>= 1) {
+                            const bool upper = (lane & off) != 0;
+#pragma unroll
+                            for (int k = 0; k < off; ++k) {
+                                const float send = upper ? v[k] : v[k + off];
+                                const float keep = upper ? v[k + off] : v[k];
+                                v[k] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+                            }
+                        }
+                        if (nb + lane < P.Cout) atomicAdd(P.colsum + nb + lane, v[0]);
+                    }
                 }
             }
         }

@@ -170,6 +170,19 @@ __device__ __forceinline__ void with_count(const int n, F&& f) {
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// per-thread register count of the calling warpgroup, lowered or raised at run time (all its warps execute it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+// counts the calling warp towards named barrier `id` without waiting for it; threads in bar.sync complete it
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // Row layout of an accumulator block for the epilogues: thread (warp w of warpgroup g, lane l) receives row
 // (w & 1) * 32 + l of g's 64x64 block, columns (w >> 1) * 32 .. + 31.  The NWG warpgroups of the CTA take turns on one
@@ -194,6 +207,33 @@ __device__ __forceinline__ void wg_rows(const float (&d)[32], float* buf, const 
         for (int q = 0; q < 8; ++q) {
             const float4 v = *reinterpret_cast<const float4*>(src + 4 * q);
             out[4 * q] = v.x; out[4 * q + 1] = v.y; out[4 * q + 2] = v.z; out[4 * q + 3] = v.w;
+        }
+    }
+}
+// The same row layout for a warpgroup whose epilogue runs out of phase with the other's (conv_planes_kernel's
+// ping-pong schedule): each warpgroup owns a 32 x kRowsPitch buffer (two of them take kRowsBytes) and named barrier
+// `bar`, and passes the 64x64 block through it in two halves of 32 rows.  Warps 2h, 2h+1 of the group write half h,
+// warps h, h+2 read it.
+__device__ __forceinline__ void wg_rows_own(const float (&d)[32], float* buf, const int bar, float (&out)[32]) {
+    const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+        named_bar_sync(bar, 128);                   // the previous half has been read
+        if ((w >> 1) == h) {
+#pragma unroll
+            for (int i = 0; i < 32; i += 2) {
+                const int row = 16 * (w & 1) + (lane >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(buf + row * kRowsPitch + col) = make_float2(d[i], d[i + 1]);
+            }
+        }
+        named_bar_sync(bar, 128);
+        if ((w & 1) == h) {
+            const float* src = buf + lane * kRowsPitch + (w >> 1) * 32;
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+                const float4 v = *reinterpret_cast<const float4*>(src + 4 * q);
+                out[4 * q] = v.x; out[4 * q + 1] = v.y; out[4 * q + 2] = v.z; out[4 * q + 3] = v.w;
+            }
         }
     }
 }

@@ -1,7 +1,8 @@
 """Micro-benchmark of the RetinaHead convolutions as models/_ops.py::RetinaHeadPlanesFn runs them: activations and
-gradients as bf16 hi/lo planes, every layer one launch over the five pyramid levels, through the C ABI.  Two shapes:
-a 256->256 tower layer and the 256->720 class conv (9 anchors x 80 classes), each in three directions:
-  fwd    conv_planes_multi, bias + activation (tower: ReLU into planes; class conv: sigmoid into fp32)
+gradients as bf16 hi/lo planes, every layer one launch over the five pyramid levels, through the C ABI.  Three shapes:
+a 256->256 tower layer, the 256->720 class conv (9 anchors x 80 classes) and a 64->64 BiFPN node conv (D0 width, the
+64-column tile of conv_planes_kernel), each in three directions:
+  fwd    conv_planes_multi, bias + activation (tower, BiFPN node: ReLU into planes; class conv: sigmoid into fp32)
   dgrad  conv_planes_multi on the gradient planes, ReLU mask of the layer input, column sums (bias gradient) -> planes
   wgrad  wgrad_planes_multi from the input and gradient planes
 Times are CUDA events around `iters` back-to-back launches; TFLOP/s are algorithmic (2 * pixels * 9 * Cin * Cout per
@@ -108,7 +109,7 @@ def timed(fn):
 card = subprocess.run(['nvidia-smi', '-i', str(dev.index or 0), '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
                       capture_output=True, text=True).stdout.strip()
 print('levels', sides, 'B', B, 'pixels', px, 'iters', iters, 'mode', mode, 'card', card)
-for Cin, Cout, act in ((256, 256, N.ACT_RELU), (256, 720, N.ACT_SIGMOID)):
+for Cin, Cout, act in ((256, 256, N.ACT_RELU), (256, 720, N.ACT_SIGMOID), (64, 64, N.ACT_RELU)):
     fns, checksum = shape(Cin, Cout, act)
     flops = 2.0 * px * 9 * Cin * Cout
     for name in ('fwd', 'dgrad', 'wgrad'):
