@@ -1,5 +1,7 @@
 // Inference post-processing on the device: box decode + clip + per-anchor class max + score
-// threshold + sort + greedy NMS, for image 0 (the reference is batch-1 at inference).
+// threshold + sort + greedy NMS, for a batch of B images.  Every stage covers the whole batch in
+// one set of launches, and the per-image counts stay in device memory, so the launches can be
+// captured in a CUDA graph.  The single-image entry points run the same kernels with B = 1.
 // Reference: models/module.py:24-49 (BBoxTransform), :57-67 (ClipBoxes),
 //            models/efficientdet.py:70-86 (threshold, nms, gather), torchvision.ops.nms.
 // Bit-exactness rules (the keep-set must equal torchvision's): fp32 IoU from separately rounded
@@ -14,7 +16,7 @@ __device__ __forceinline__ uint32_t float_order(float f) {  // monotone float ->
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
-// one warp per anchor (coalesced over classes); anchors >= A emit sentinel keys
+// one warp per anchor (coalesced over classes), blockIdx.y = image; anchors >= A emit sentinel keys
 __global__ void __launch_bounds__(256) detect_candidates_kernel(const float* __restrict__ cls, const float* __restrict__ reg,
                                                                 const float* __restrict__ anchors, float* __restrict__ boxes,
                                                                 float* __restrict__ scores, int32_t* __restrict__ classes,
@@ -23,11 +25,14 @@ __global__ void __launch_bounds__(256) detect_candidates_kernel(const float* __r
                                                                 float threshold) {
     const int lane = threadIdx.x & 31;
     const int a = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const long long b = blockIdx.y;
     if (a >= npad) return;
+    keys += b * npad;
     if (a >= A) {
         if (lane == 0) keys[a] = ~0ull;
         return;
     }
+    cls += b * A * K;
     float best = -INFINITY;
     int arg = 0x7fffffff;
     for (int k = lane; k < K; k += 32) {
@@ -42,7 +47,7 @@ __global__ void __launch_bounds__(256) detect_candidates_kernel(const float* __r
     }
     if (lane != 0) return;
     const float4 an = ldg4(anchors + (long long)a * 4);
-    const float4 d = ldg4(reg + (long long)a * 4);
+    const float4 d = ldg4(reg + (b * A + a) * 4);
     const float w = __fsub_rn(an.z, an.x), h = __fsub_rn(an.w, an.y);
     const float cx = __fadd_rn(an.x, __fmul_rn(0.5f, w)), cy = __fadd_rn(an.y, __fmul_rn(0.5f, h));
     const float dx = __fadd_rn(__fmul_rn(d.x, 0.1f), 0.f), dy = __fadd_rn(__fmul_rn(d.y, 0.1f), 0.f);
@@ -53,26 +58,31 @@ __global__ void __launch_bounds__(256) detect_candidates_kernel(const float* __r
     float x2 = __fadd_rn(pcx, __fmul_rn(0.5f, pw)), y2 = __fadd_rn(pcy, __fmul_rn(0.5f, ph));
     x1 = fmaxf(x1, 0.f); y1 = fmaxf(y1, 0.f);
     x2 = fminf(x2, img_w); y2 = fminf(y2, img_h);
-    st4(boxes + (long long)a * 4, make_float4(x1, y1, x2, y2));
-    scores[a] = best;
-    classes[a] = arg;
+    st4(boxes + (b * A + a) * 4, make_float4(x1, y1, x2, y2));
+    scores[b * A + a] = best;
+    classes[b * A + a] = arg;
     if (best > threshold) {
         keys[a] = ((uint64_t)(~float_order(best)) << 32) | (uint32_t)a;
-        atomicAdd(count, 1);
+        atomicAdd(count + b, 1);
     } else {
         keys[a] = ~0ull;
     }
 }
 
-// ---- bitonic sort of 64-bit keys (ascending); n is a power of two >= 2048 or handled as one chunk ----
+// ---- bitonic sort of 64-bit keys (ascending) in independent segments of `seg` keys (a power of two) ----
+// The keys of all segments form one array; every compare-exchange stays inside its segment because j < k <= seg.
+// The direction of stage k comes from the index inside the segment: at k == seg the global index would alternate it
+// from one segment to the next.
 constexpr int kChunk = 2048;
 
 __device__ __forceinline__ void cmpswap(uint64_t& a, uint64_t& b, bool asc) {
     if ((a > b) == asc) { const uint64_t t = a; a = b; b = t; }
 }
 
-// sorts every aligned chunk (stages k = 2 .. chunk) with the direction given by the global index
-__global__ void __launch_bounds__(1024) bitonic_chunk_sort_kernel(uint64_t* __restrict__ keys, int chunk) {
+__device__ __forceinline__ bool bitonic_asc(int i, int seg, int k) { return ((i & (seg - 1)) & k) == 0; }
+
+// sorts every aligned chunk (stages k = 2 .. chunk); chunk <= seg
+__global__ void __launch_bounds__(1024) bitonic_chunk_sort_kernel(uint64_t* __restrict__ keys, int chunk, int seg) {
     extern __shared__ uint64_t sk[];
     const int base = blockIdx.x * chunk;
     for (int i = threadIdx.x; i < chunk; i += blockDim.x) sk[i] = keys[base + i];
@@ -81,8 +91,7 @@ __global__ void __launch_bounds__(1024) bitonic_chunk_sort_kernel(uint64_t* __re
         for (int j = k >> 1; j > 0; j >>= 1) {
             for (int t = threadIdx.x; t < chunk / 2; t += blockDim.x) {
                 const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-                const bool asc = (((base + i) & k) == 0);
-                cmpswap(sk[i], sk[i | j], asc);
+                cmpswap(sk[i], sk[i | j], bitonic_asc(base + i, seg, k));
             }
             __syncthreads();
         }
@@ -90,17 +99,17 @@ __global__ void __launch_bounds__(1024) bitonic_chunk_sort_kernel(uint64_t* __re
     for (int i = threadIdx.x; i < chunk; i += blockDim.x) keys[base + i] = sk[i];
 }
 
-__global__ void __launch_bounds__(256) bitonic_global_step_kernel(uint64_t* __restrict__ keys, int n, int k, int j) {
+__global__ void __launch_bounds__(256) bitonic_global_step_kernel(uint64_t* __restrict__ keys, int n, int seg, int k, int j) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n / 2) return;
     const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-    const bool asc = ((i & k) == 0);
+    const bool asc = bitonic_asc(i, seg, k);
     uint64_t a = keys[i], b = keys[i | j];
     if ((a > b) == asc) { keys[i] = b; keys[i | j] = a; }
 }
 
 // finishes stage k inside each chunk: j = chunk/2 .. 1
-__global__ void __launch_bounds__(1024) bitonic_chunk_merge_kernel(uint64_t* __restrict__ keys, int chunk, int k) {
+__global__ void __launch_bounds__(1024) bitonic_chunk_merge_kernel(uint64_t* __restrict__ keys, int chunk, int seg, int k) {
     extern __shared__ uint64_t sk[];
     const int base = blockIdx.x * chunk;
     for (int i = threadIdx.x; i < chunk; i += blockDim.x) sk[i] = keys[base + i];
@@ -108,8 +117,7 @@ __global__ void __launch_bounds__(1024) bitonic_chunk_merge_kernel(uint64_t* __r
     for (int j = chunk >> 1; j > 0; j >>= 1) {
         for (int t = threadIdx.x; t < chunk / 2; t += blockDim.x) {
             const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-            const bool asc = (((base + i) & k) == 0);
-            cmpswap(sk[i], sk[i | j], asc);
+            cmpswap(sk[i], sk[i | j], bitonic_asc(base + i, seg, k));
         }
         __syncthreads();
     }
@@ -130,35 +138,86 @@ __device__ __forceinline__ bool iou_gt(const float4 a, const float4 b, double th
     return (double)ovr > thr;
 }
 
-// mask[i][cb] bit j set  <=>  sorted box (64*cb + j) is suppressed by sorted box i  (upper triangle only)
-__global__ void __launch_bounds__(64) nms_mask_kernel(const float* __restrict__ boxes, const uint64_t* __restrict__ keys,
-                                                      int n, double thr, uint64_t* __restrict__ mask) {
-    const int rb = blockIdx.y, cb = blockIdx.x;
-    if (rb > cb) return;
-    const int col_blocks = (n + 63) / 64;
-    __shared__ float4 cbx[64];
-    const int cj = cb * 64 + threadIdx.x;
-    if (cj < n) cbx[threadIdx.x] = ldg4(boxes + (long long)(uint32_t)keys[cj] * 4);
-    __syncthreads();
-    const int i = rb * 64 + threadIdx.x;
-    if (i >= n) return;
-    const float4 me = ldg4(boxes + (long long)(uint32_t)keys[i] * 4);
-    const int csize = min(64, n - cb * 64);
-    uint64_t bits = 0;
-    for (int j = (rb == cb ? threadIdx.x + 1 : 0); j < csize; ++j)
-        if (iou_gt(me, cbx[j], thr)) bits |= 1ull << j;
-    mask[(long long)i * col_blocks + cb] = bits;
+// Candidates NMS works on in image b: count[b] (all `cap` when count is NULL), or 0 when count[b] > cap (overflow).
+__device__ __forceinline__ int nms_candidates(const int32_t* count, int b, int cap) {
+    const int n = count ? count[b] : cap;
+    return n > cap ? 0 : n;
 }
 
-// Greedy scan over the sorted candidates, one CTA; the `removed` bitmap lives in shared memory.  Candidates are
+// Persistent over the upper-triangle 64x64 tiles of all B images, numbered image by image and row by row inside an
+// image (row rb holds tiles cb = rb .. cw_b-1, cw_b = ceil(n_b/64)).  The grid depends on B and cap only.  Each CTA
+// walks that numbering forward as its tile index grows, so the walk costs O(B + rows) per CTA in total.
+// mask[b][i][cb] bit j set  <=>  sorted box (64*cb + j) of image b is suppressed by its sorted box i; row stride ceil(cap/64).
+__global__ void __launch_bounds__(64) nms_mask_kernel(const float* __restrict__ boxes, const uint64_t* __restrict__ keys,
+                                                      const int32_t* __restrict__ count, int B, int A, int npad, int cap,
+                                                      double thr, uint64_t* __restrict__ mask) {
+    __shared__ float4 cbx[64];
+    const int cw_cap = (cap + 63) / 64;
+    int b = 0, n = nms_candidates(count, 0, cap), cw = (n + 63) / 64;
+    long long img_base = 0, img_tiles = (long long)cw * (cw + 1) / 2;   // first tile of image b, tiles of image b
+    int rb = 0;
+    long long row_base = 0;                                            // first tile of row rb, relative to img_base
+    for (long long t = blockIdx.x;; t += gridDim.x) {
+        while (t >= img_base + img_tiles) {
+            img_base += img_tiles;
+            if (++b >= B) return;
+            n = nms_candidates(count, b, cap);
+            cw = (n + 63) / 64;
+            img_tiles = (long long)cw * (cw + 1) / 2;
+            rb = 0;
+            row_base = 0;
+        }
+        const long long local = t - img_base;
+        while (local >= row_base + (cw - rb)) {
+            row_base += cw - rb;
+            ++rb;
+        }
+        const int cb = rb + (int)(local - row_base);
+        const uint64_t* kb = keys + (long long)b * npad;
+        const float* bx = boxes + (long long)b * A * 4;
+        const int cj = cb * 64 + threadIdx.x;
+        if (cj < n) cbx[threadIdx.x] = ldg4(bx + (long long)(uint32_t)kb[cj] * 4);
+        __syncthreads();
+        const int i = rb * 64 + threadIdx.x;
+        if (i < n) {
+            const float4 me = ldg4(bx + (long long)(uint32_t)kb[i] * 4);
+            const int csize = min(64, n - cb * 64);
+            uint64_t bits = 0;
+            if (rb != cb && csize == 64) {             // almost every tile: fixed trip count, constant bit positions
+#pragma unroll 8
+                for (int j = 0; j < 64; ++j)
+                    if (iou_gt(me, cbx[j], thr)) bits |= 1ull << j;
+            } else {
+                for (int j = (rb == cb ? threadIdx.x + 1 : 0); j < csize; ++j)
+                    if (iou_gt(me, cbx[j], thr)) bits |= 1ull << j;
+            }
+            mask[((long long)b * cap + i) * cw_cap + cb] = bits;
+        }
+        __syncthreads();
+    }
+}
+
+// Greedy scan over the sorted candidates, one CTA per image; the `removed` bitmap lives in shared memory.  Candidates are
 // consumed 64 at a time: warp 0 resolves the block's internal dependencies from the 64 diagonal mask words (a
 // sequential walk over 64 bits, registers + shuffles only), then every thread ORs the rows of the block's survivors
 // into its slice of `removed`.  Two CTA barriers per 64 candidates instead of two per kept box: the scan used to be
 // 255 ms for the 55 k survivors of a random-weight D7 image.  Result identical to the one-at-a-time scan.
+// nkeep[b] = kept boxes, or -1 when count[b] > cap (nothing else is written for that image).
 __global__ void __launch_bounds__(1024) nms_scan_kernel(const uint64_t* __restrict__ mask, const uint64_t* __restrict__ keys,
-                                                        int n, int32_t* __restrict__ keep_idx, int32_t* __restrict__ nkeep) {
+                                                        const int32_t* __restrict__ count, int npad, int cap,
+                                                        int32_t* __restrict__ keep_idx, int32_t* __restrict__ nkeep) {
     extern __shared__ uint64_t removed[];
     __shared__ uint64_t keep_bits;
+    const int b = blockIdx.x;
+    const int n = count ? count[b] : cap;
+    if (n > cap) {
+        if (threadIdx.x == 0) nkeep[b] = -1;
+        return;
+    }
+    const int cw_cap = (cap + 63) / 64;
+    mask += (long long)b * cap * cw_cap;
+    keys += (long long)b * npad;
+    keep_idx += (long long)b * cap;
     const int col_blocks = (n + 63) / 64;
     const int lane = threadIdx.x & 31;
     for (int j = threadIdx.x; j < col_blocks; j += blockDim.x) removed[j] = 0;
@@ -167,15 +226,15 @@ __global__ void __launch_bounds__(1024) nms_scan_kernel(const uint64_t* __restri
     for (int nb = 0; nb < col_blocks; ++nb) {
         if (threadIdx.x < 32) {
             const int i0 = nb * 64 + lane, i1 = i0 + 32;
-            const uint64_t d0 = i0 < n ? mask[(long long)i0 * col_blocks + nb] : 0ull;     // bits j > i inside the block
-            const uint64_t d1 = i1 < n ? mask[(long long)i1 * col_blocks + nb] : 0ull;
+            const uint64_t d0 = i0 < n ? mask[(long long)i0 * cw_cap + nb] : 0ull;     // bits j > i inside the block
+            const uint64_t d1 = i1 < n ? mask[(long long)i1 * cw_cap + nb] : 0ull;
             uint64_t rem = removed[nb], kb = 0;
             const int valid = min(64, n - nb * 64);
 #pragma unroll 1
-            for (int b = 0; b < valid; ++b) {
-                const uint64_t row = __shfl_sync(0xffffffffu, b < 32 ? d0 : d1, b & 31);
-                if (!((rem >> b) & 1ull)) {
-                    kb |= 1ull << b;
+            for (int bit = 0; bit < valid; ++bit) {
+                const uint64_t row = __shfl_sync(0xffffffffu, bit < 32 ? d0 : d1, bit & 31);
+                if (!((rem >> bit) & 1ull)) {
+                    kb |= 1ull << bit;
                     rem |= row;
                 }
             }
@@ -188,28 +247,92 @@ __global__ void __launch_bounds__(1024) nms_scan_kernel(const uint64_t* __restri
         for (int j = nb + 1 + threadIdx.x; j < col_blocks; j += blockDim.x) {
             uint64_t acc = 0, bits = kb;
             while (bits) {
-                const int b = __ffsll((long long)bits) - 1;
+                const int bit = __ffsll((long long)bits) - 1;
                 bits &= bits - 1;
-                acc |= mask[(long long)(nb * 64 + b) * col_blocks + j];
+                acc |= mask[(long long)(nb * 64 + bit) * cw_cap + j];
             }
             removed[j] |= acc;
         }
         kept += __popcll(kb);
         __syncthreads();
     }
-    if (threadIdx.x == 0) nkeep[0] = kept;
+    if (threadIdx.x == 0) nkeep[b] = kept;
 }
 
+// row i of image b (blockIdx.y): the i-th kept detection, zero from nkeep[b] on (all `cap` rows kept when nkeep is NULL)
 __global__ void gather_detections_kernel(const float* __restrict__ boxes, const float* __restrict__ scores,
-                                         const int32_t* __restrict__ classes, const int32_t* __restrict__ keep_idx, int nkeep,
-                                         float* __restrict__ out_scores, long long* __restrict__ out_classes,
-                                         float* __restrict__ out_boxes) {
+                                         const int32_t* __restrict__ classes, const int32_t* __restrict__ keep_idx,
+                                         const int32_t* __restrict__ nkeep, int A, int cap, float* __restrict__ out_scores,
+                                         long long* __restrict__ out_classes, float* __restrict__ out_boxes) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nkeep) return;
-    const int a = keep_idx[i];
-    out_scores[i] = scores[a];
-    out_classes[i] = (long long)classes[a];
-    st4(out_boxes + (long long)i * 4, ldg4(boxes + (long long)a * 4));
+    const long long b = blockIdx.y;
+    if (i >= cap) return;
+    const long long o = b * cap + i;
+    const int m = nkeep ? nkeep[b] : cap;
+    if (i < m) {
+        const long long a = b * A + keep_idx[o];
+        out_scores[o] = scores[a];
+        out_classes[o] = (long long)classes[a];
+        st4(out_boxes + o * 4, ldg4(boxes + a * 4));
+    } else {
+        out_scores[o] = 0.f;
+        out_classes[o] = 0;
+        st4(out_boxes + o * 4, f4zero());
+    }
+}
+
+constexpr size_t kScanSmemLimit = 200 * 1024;
+
+static int candidates_launch(const float* cls, const float* reg, const float* anchors, float* boxes, float* scores,
+                             int32_t* classes, uint64_t* keys, int32_t* count, int B, int A, int K, int npad, float img_w,
+                             float img_h, float threshold, cudaStream_t st) {
+    cudaError_t e = cudaMemsetAsync(count, 0, (size_t)B * sizeof(int32_t), st);
+    if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "detect_candidates: memset: %s", cudaGetErrorString(e));
+    detect_candidates_kernel<<<dim3(cdiv(npad, 8), B), 256, 0, st>>>(cls, reg, anchors, boxes, scores, classes, keys, count, A,
+                                                                    K, npad, img_w, img_h, threshold);
+    int s = launch_status("detect_candidates_kernel");
+    if (s) return s;
+    // sort every image's segment ascending: best candidates first, sentinels last
+    const int n = B * npad;
+    const int chunk = npad < kChunk ? npad : kChunk;
+    if (chunk >= 2) {
+        bitonic_chunk_sort_kernel<<<n / chunk, 1024, chunk * sizeof(uint64_t), st>>>(keys, chunk, npad);
+        if ((s = launch_status("bitonic_chunk_sort_kernel"))) return s;
+    }
+    for (int k = chunk * 2; k <= npad; k <<= 1) {
+        for (int j = k >> 1; j >= chunk; j >>= 1) {
+            bitonic_global_step_kernel<<<cdiv(n / 2, 256), 256, 0, st>>>(keys, n, npad, k, j);
+            if ((s = launch_status("bitonic_global_step_kernel"))) return s;
+        }
+        bitonic_chunk_merge_kernel<<<n / chunk, 1024, chunk * sizeof(uint64_t), st>>>(keys, chunk, npad, k);
+        if ((s = launch_status("bitonic_chunk_merge_kernel"))) return s;
+    }
+    return EFFDET_OK;
+}
+
+static int nms_launch(const float* boxes, const uint64_t* keys, const int32_t* count, int B, int A, int npad, int cap,
+                      double iou_threshold, uint64_t* mask_ws, int32_t* keep_idx, int32_t* nkeep, cudaStream_t st) {
+    const long long cw = cdiv(cap, 64);
+    const long long tiles = (long long)B * (cw * (cw + 1) / 2);        // upper bound: every image at `cap` candidates
+    const int grid = (int)(tiles < (long long)num_sms() * 32 ? tiles : (long long)num_sms() * 32);
+    nms_mask_kernel<<<grid, 64, 0, st>>>(boxes, keys, count, B, A, npad, cap, iou_threshold, mask_ws);
+    int s = launch_status("nms_mask_kernel");
+    if (s) return s;
+    const size_t smem = (size_t)cw * sizeof(uint64_t);
+    if (smem > 48 * 1024) {
+        cudaError_t e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "nms: smem opt-in: %s", cudaGetErrorString(e));
+    }
+    nms_scan_kernel<<<B, 1024, smem, st>>>(mask_ws, keys, count, npad, cap, keep_idx, nkeep);
+    return launch_status("nms_scan_kernel");
+}
+
+static int gather_launch(const float* boxes, const float* scores, const int32_t* classes, const int32_t* keep_idx,
+                         const int32_t* nkeep, int B, int A, int cap, float* out_scores, int64_t* out_classes,
+                         float* out_boxes, cudaStream_t st) {
+    gather_detections_kernel<<<dim3(cdiv(cap, 256), B), 256, 0, st>>>(boxes, scores, classes, keep_idx, nkeep, A, cap,
+                                                                      out_scores, (long long*)out_classes, out_boxes);
+    return launch_status("gather_detections_kernel");
 }
 
 }  // namespace effdet
@@ -224,48 +347,16 @@ extern "C" int effdet_detect_candidates(const float* cls, const float* reg, cons
     EFFDET_REQUIRE(A > 0 && K > 0 && npad >= A && (npad & (npad - 1)) == 0, "detect_candidates: npad must be a power of two >= A");
     EFFDET_REQUIRE(aligned16(reg) && aligned16(anchors) && aligned16(boxes), "detect_candidates: alignment");
     EFFDET_DEVICE(device);
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaMemsetAsync(count, 0, sizeof(int32_t), st);
-    if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "detect_candidates: memset: %s", cudaGetErrorString(e));
-    detect_candidates_kernel<<<cdiv(npad, 8), 256, 0, st>>>(cls, reg, anchors, boxes, scores, classes, keys, count, A, K, npad,
-                                                           img_w, img_h, threshold);
-    int s = launch_status("detect_candidates_kernel");
-    if (s) return s;
-    // sort ascending: best candidates first, sentinels last
-    const int chunk = npad < kChunk ? npad : kChunk;
-    if (chunk >= 2) {
-        bitonic_chunk_sort_kernel<<<npad / chunk, 1024, chunk * sizeof(uint64_t), st>>>(keys, chunk);
-        if ((s = launch_status("bitonic_chunk_sort_kernel"))) return s;
-    }
-    for (int k = chunk * 2; k <= npad; k <<= 1) {
-        for (int j = k >> 1; j >= chunk; j >>= 1) {
-            bitonic_global_step_kernel<<<cdiv(npad / 2, 256), 256, 0, st>>>(keys, npad, k, j);
-            if ((s = launch_status("bitonic_global_step_kernel"))) return s;
-        }
-        bitonic_chunk_merge_kernel<<<npad / chunk, 1024, chunk * sizeof(uint64_t), st>>>(keys, chunk, k);
-        if ((s = launch_status("bitonic_chunk_merge_kernel"))) return s;
-    }
-    return EFFDET_OK;
+    return candidates_launch(cls, reg, anchors, boxes, scores, classes, keys, count, 1, A, K, npad, img_w, img_h, threshold,
+                             (cudaStream_t)stream);
 }
 
 extern "C" int effdet_nms(const float* boxes, const uint64_t* keys, int n, double iou_threshold, uint64_t* mask_ws,
                           int32_t* keep_idx, int32_t* nkeep, int device, effdet_stream_t stream) {
     EFFDET_REQUIRE(boxes && keys && mask_ws && keep_idx && nkeep && n > 0, "nms: bad arguments");
+    EFFDET_REQUIRE((size_t)cdiv(n, 64) * sizeof(uint64_t) <= kScanSmemLimit, "nms: too many candidates for the scan bitmap (%d)", n);
     EFFDET_DEVICE(device);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int col_blocks = cdiv(n, 64);
-    EFFDET_REQUIRE(col_blocks <= 65535, "nms: too many candidates (%d)", n);
-    const size_t smem = (size_t)col_blocks * sizeof(uint64_t);
-    EFFDET_REQUIRE(smem <= 200 * 1024, "nms: too many candidates for the scan bitmap (%d)", n);
-    nms_mask_kernel<<<dim3(col_blocks, col_blocks), 64, 0, st>>>(boxes, keys, n, iou_threshold, mask_ws);
-    int s = launch_status("nms_mask_kernel");
-    if (s) return s;
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "nms: smem opt-in: %s", cudaGetErrorString(e));
-    }
-    nms_scan_kernel<<<1, 1024, smem, st>>>(mask_ws, keys, n, keep_idx, nkeep);
-    return launch_status("nms_scan_kernel");
+    return nms_launch(boxes, keys, nullptr, 1, 0, 0, n, iou_threshold, mask_ws, keep_idx, nkeep, (cudaStream_t)stream);
 }
 
 extern "C" int effdet_gather_detections(const float* boxes, const float* scores, const int32_t* classes,
@@ -275,8 +366,50 @@ extern "C" int effdet_gather_detections(const float* boxes, const float* scores,
                    "gather_detections: bad arguments");
     EFFDET_REQUIRE(aligned16(boxes) && aligned16(out_boxes), "gather_detections: alignment");
     EFFDET_DEVICE(device);
-    gather_detections_kernel<<<cdiv(nkeep, 256), 256, 0, (cudaStream_t)stream>>>(boxes, scores, classes, keep_idx, nkeep,
-                                                                               out_scores, (long long*)out_classes,
-                                                                               out_boxes);
-    return launch_status("gather_detections_kernel");
+    return gather_launch(boxes, scores, classes, keep_idx, nullptr, 1, 0, nkeep, out_scores, out_classes, out_boxes,
+                         (cudaStream_t)stream);
+}
+
+extern "C" int effdet_detect_candidates_batch(const float* cls, const float* reg, const float* anchors, float* boxes,
+                                              float* scores, int32_t* classes, uint64_t* keys, int32_t* count, int B, int A,
+                                              int K, int npad, float img_w, float img_h, float threshold, int device,
+                                              effdet_stream_t stream) {
+    EFFDET_REQUIRE(cls && reg && anchors && boxes && scores && classes && keys && count, "detect_candidates_batch: null tensor");
+    EFFDET_REQUIRE(B >= 1 && B <= 65535, "detect_candidates_batch: B=%d must be in [1, 65535]", B);
+    EFFDET_REQUIRE(A > 0 && K > 0 && npad >= A && (npad & (npad - 1)) == 0,
+                   "detect_candidates_batch: npad=%d must be a power of two >= A=%d (K=%d > 0)", npad, A, K);
+    EFFDET_REQUIRE((long long)B * npad <= (1ll << 30), "detect_candidates_batch: B*npad = %lld keys is too many",
+                   (long long)B * npad);
+    EFFDET_REQUIRE(aligned16(reg) && aligned16(anchors) && aligned16(boxes), "detect_candidates_batch: alignment");
+    EFFDET_DEVICE(device);
+    return candidates_launch(cls, reg, anchors, boxes, scores, classes, keys, count, B, A, K, npad, img_w, img_h, threshold,
+                             (cudaStream_t)stream);
+}
+
+extern "C" int effdet_nms_batch(const float* boxes, const uint64_t* keys, const int32_t* count, int B, int A, int npad,
+                                int cap, double iou_threshold, uint64_t* mask_ws, int32_t* keep_idx, int32_t* nkeep,
+                                int device, effdet_stream_t stream) {
+    EFFDET_REQUIRE(boxes && keys && count && mask_ws && keep_idx && nkeep, "nms_batch: null tensor");
+    EFFDET_REQUIRE(B >= 1, "nms_batch: B=%d must be >= 1", B);
+    EFFDET_REQUIRE(A > 0 && npad >= A && (npad & (npad - 1)) == 0, "nms_batch: npad=%d must be a power of two >= A=%d", npad, A);
+    EFFDET_REQUIRE(cap >= 1 && cap <= A, "nms_batch: cap=%d must be in [1, A=%d]", cap, A);
+    EFFDET_REQUIRE((size_t)cdiv(cap, 64) * sizeof(uint64_t) <= kScanSmemLimit,
+                   "nms_batch: cap=%d is too large for the scan bitmap (%zu bytes of shared memory at most)", cap, kScanSmemLimit);
+    EFFDET_REQUIRE(aligned16(boxes), "nms_batch: alignment");
+    EFFDET_DEVICE(device);
+    return nms_launch(boxes, keys, count, B, A, npad, cap, iou_threshold, mask_ws, keep_idx, nkeep, (cudaStream_t)stream);
+}
+
+extern "C" int effdet_gather_detections_batch(const float* boxes, const float* scores, const int32_t* classes,
+                                              const int32_t* keep_idx, const int32_t* nkeep, int B, int A, int cap,
+                                              float* out_scores, int64_t* out_classes, float* out_boxes, int device,
+                                              effdet_stream_t stream) {
+    EFFDET_REQUIRE(boxes && scores && classes && keep_idx && nkeep && out_scores && out_classes && out_boxes,
+                   "gather_detections_batch: null tensor");
+    EFFDET_REQUIRE(B >= 1 && B <= 65535, "gather_detections_batch: B=%d must be in [1, 65535]", B);
+    EFFDET_REQUIRE(A > 0 && cap >= 1 && cap <= A, "gather_detections_batch: cap=%d must be in [1, A=%d]", cap, A);
+    EFFDET_REQUIRE(aligned16(boxes) && aligned16(out_boxes), "gather_detections_batch: alignment");
+    EFFDET_DEVICE(device);
+    return gather_launch(boxes, scores, classes, keep_idx, nkeep, B, A, cap, out_scores, out_classes, out_boxes,
+                         (cudaStream_t)stream);
 }

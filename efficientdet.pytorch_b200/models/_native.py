@@ -162,6 +162,9 @@ SIGNATURES = {
     'effdet_detect_candidates': [_P] * 8 + [_INT, _INT, _INT, _F, _F, _F] + _TAIL,
     'effdet_nms': [_P, _P, _INT, ctypes.c_double, _P, _P, _P] + _TAIL,
     'effdet_gather_detections': [_P, _P, _P, _P, _INT, _P, _P, _P] + _TAIL,
+    'effdet_detect_candidates_batch': [_P] * 8 + [_INT, _INT, _INT, _INT, _F, _F, _F] + _TAIL,
+    'effdet_nms_batch': [_P, _P, _P, _INT, _INT, _INT, _INT, ctypes.c_double, _P, _P, _P] + _TAIL,
+    'effdet_gather_detections_batch': [_P, _P, _P, _P, _P, _INT, _INT, _INT, _P, _P, _P] + _TAIL,
     'effdet_multi_sumsq': [_P, _P, _P, _P, _INT, _INT, _P] + _TAIL,
     'effdet_multi_clip_adamw': [_P] * 7 + [_INT, _INT, _P] + [_F] * 8 + [_INT] + _TAIL,
     'effdet_normalize_pad': [_P, _P, _P, _P, _P, _INT, _INT, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)] + _TAIL,

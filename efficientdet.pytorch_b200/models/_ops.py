@@ -7,6 +7,7 @@ so DDP's reducer hooks and ``clip_grad_norm_`` (reference train.py:114-116) keep
 Internal activation layout is NHWC fp32; module boundaries expose the same memory as a logical
 NCHW tensor with channels_last strides (zero-copy ``permute`` views).
 """
+import collections
 import os
 import weakref
 
@@ -1008,37 +1009,59 @@ class FocalLossFn(torch.autograd.Function):
 # ------------------------------------------------------------------------------------------------
 
 
-def detect_image0(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, index=0):
-    """-> [scores[K], classes[K] int64, boxes[K,4]] for image `index` (the reference only ever looks at image 0,
-    models/efficientdet.py:73-86), or None when nothing passes."""
-    cls0, reg0 = _contig(cls[index]), _contig(reg[index])
-    A, K = cls0.shape
+# Bytes the eager NMS mask workspace may take before the batch is split into consecutive groups of images (at least one
+# image per group).  Realistic candidate counts keep the whole batch in one group: 5 k candidates cost 3.2 MB per image.
+NMS_MASK_BUDGET = 1 << 30
+
+Detections = collections.namedtuple('Detections', 'scores classes boxes count')
+
+
+def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=None):
+    """Decode + clip + class max + threshold + greedy NMS of every image of cls [B,A,K] / reg [B,A,4], one set of
+    launches for the whole batch (the reference does this for image 0 only, models/efficientdet.py:73-86).
+
+    cap=None: reads the B candidate counts once to set cap = their maximum and the B kept counts once to slice the
+    results -> list of B triples [scores[K_b], classes[K_b] int64, boxes[K_b,4]] on the device (empty tensors when no
+    anchor passes the threshold).
+    cap=C: no host synchronisation, so the call can be captured in a CUDA graph -> Detections(scores [B,C],
+    classes [B,C] int64, boxes [B,C,4], count [B] int32), rows past count[b] zero; count[b] == -1 when image b has
+    more than C candidates (its rows are then all zero)."""
+    check_cuda_f32(cls, 'classifications')
+    check_cuda_f32(reg, 'regressions')
+    cls, reg = _contig(cls), _contig(reg)
+    B, A, K = cls.shape
     anchors = _contig(anchors.view(-1, 4))
-    npad = 1
-    while npad < A:
-        npad *= 2
-    dev = cls0.device
-    boxes = _empty((A, 4), cls0)
-    scores = _empty((A,), cls0)
-    classes = torch.empty((A,), device=dev, dtype=torch.int32)
-    keys = torch.empty((npad,), device=dev, dtype=torch.int64)
-    count = torch.empty((1,), device=dev, dtype=torch.int32)
-    N.call('effdet_detect_candidates', cls0, N.f32(cls0), N.f32(reg0), N.f32(anchors), N.f32(boxes), N.f32(scores),
-           classes.data_ptr(), keys.data_ptr(), count.data_ptr(), A, K, npad, float(img_w), float(img_h),
+    npad = 1 << (A - 1).bit_length()
+    dev = cls.device
+    boxes = _empty((B, A, 4), cls)
+    scores = _empty((B, A), cls)
+    classes = torch.empty((B, A), device=dev, dtype=torch.int32)
+    keys = torch.empty((B, npad), device=dev, dtype=torch.int64)
+    count = torch.empty((B,), device=dev, dtype=torch.int32)
+    N.call('effdet_detect_candidates_batch', cls, N.f32(cls), N.f32(reg), N.f32(anchors), N.f32(boxes), N.f32(scores),
+           classes.data_ptr(), keys.data_ptr(), count.data_ptr(), B, A, K, npad, float(img_w), float(img_h),
            float(threshold))
-    n = int(count.item())                       # host reads one int to size the NMS workspace
-    if n == 0:
-        return None
-    cb = (n + 63) // 64
-    mask = torch.empty((n * cb,), device=dev, dtype=torch.int64)
-    keep = torch.empty((n,), device=dev, dtype=torch.int32)
-    nkeep = torch.empty((1,), device=dev, dtype=torch.int32)
-    N.call('effdet_nms', cls0, N.f32(boxes), keys.data_ptr(), n, float(iou_threshold), mask.data_ptr(),
-           keep.data_ptr(), nkeep.data_ptr())
-    m = int(nkeep.item())
-    o_s = _empty((m,), cls0)
-    o_c = torch.empty((m,), device=dev, dtype=torch.int64)
-    o_b = _empty((m, 4), cls0)
-    N.call('effdet_gather_detections', cls0, N.f32(boxes), N.f32(scores), classes.data_ptr(), keep.data_ptr(), m,
-           N.f32(o_s), o_c.data_ptr(), N.f32(o_b))
-    return [o_s, o_c, o_b]
+    eager = cap is None
+    if eager:
+        cap = int(count.max().item())                # host read 1 of 2: sizes the NMS workspace and the outputs
+        if cap == 0:
+            return [[cls.new_zeros(0), torch.zeros(0, dtype=torch.int64, device=dev), cls.new_zeros(0, 4)]
+                    for _ in range(B)]
+    cw = (cap + 63) // 64
+    per_image = cap * cw * 8
+    group = min(B, max(NMS_MASK_BUDGET, per_image) // per_image)
+    mask = torch.empty((group * cap * cw,), device=dev, dtype=torch.int64)
+    keep = torch.empty((B, cap), device=dev, dtype=torch.int32)
+    nkeep = torch.empty((B,), device=dev, dtype=torch.int32)
+    for b0 in range(0, B, group):
+        N.call('effdet_nms_batch', cls, N.f32(boxes[b0:]), keys[b0:].data_ptr(), count[b0:].data_ptr(), min(group, B - b0),
+               A, npad, cap, float(iou_threshold), mask.data_ptr(), keep[b0:].data_ptr(), nkeep[b0:].data_ptr())
+    o_s = _empty((B, cap), cls)
+    o_c = torch.empty((B, cap), device=dev, dtype=torch.int64)
+    o_b = _empty((B, cap, 4), cls)
+    N.call('effdet_gather_detections_batch', cls, N.f32(boxes), N.f32(scores), classes.data_ptr(), keep.data_ptr(),
+           nkeep.data_ptr(), B, A, cap, N.f32(o_s), o_c.data_ptr(), N.f32(o_b))
+    if not eager:
+        return Detections(o_s, o_c, o_b, nkeep)
+    m = nkeep.tolist()                               # host read 2 of 2
+    return [[o_s[b, :m[b]], o_c[b, :m[b]], o_b[b, :m[b]]] for b in range(B)]

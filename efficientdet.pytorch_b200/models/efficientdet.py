@@ -6,7 +6,7 @@ around sm_90a kernels.  Same constructor, attributes, call convention and state-
 
 What differs underneath: features stay NHWC end to end, the head writes the level-concatenated
 ``[B, sum(HWA), K]`` / ``[B, sum(HWA), 4]`` tensors directly (no ``torch.cat``), anchors are cached per input
-size, and decode + clip + threshold + NMS run on the device with two scalar read-backs.
+size, and decode + clip + threshold + NMS run on the device for the whole batch with two read-backs.
 """
 import math
 
@@ -90,9 +90,9 @@ class EfficientDet(nn.Module):
 
     def _detections(self, image):
         cls, reg, anchors = self._raw_predictions(image)
-        found = _ops.detect_image0(cls, reg, anchors, image.shape[2], image.shape[3], self.threshold,
-                                   self.iou_threshold)
-        if found is None:
+        found = _ops.detect_batch(cls[:1], reg[:1], anchors, image.shape[2], image.shape[3], self.threshold,
+                                  self.iou_threshold)[0]
+        if found[0].numel() == 0:
             print('No boxes to NMS')
             return [torch.zeros(0), torch.zeros(0), torch.zeros(0, 4)]
         return found
@@ -109,20 +109,14 @@ class EfficientDet(nn.Module):
     @torch.no_grad()
     def detect_batch(self, images):
         """Batched inference (SURVEY.md 8(f) rank 3): one network pass over [B,3,H,W], then decode + threshold +
-        NMS per image.  The reference's forward only post-processes image 0 (models/efficientdet.py:73-86), which
-        is why eval.py feeds it one image at a time; entry i here equals forward(images[i:i+1]).
+        NMS of all B images in one set of launches and two host reads.  The reference's forward only post-processes
+        image 0 (models/efficientdet.py:73-86), which is why eval.py feeds it one image at a time; entry i here equals
+        forward(images[i:i+1]).
         -> list of B triples [scores[K_i], classes[K_i] int64, boxes[K_i,4]] on the device (empty tensors when no
         anchor passes the threshold)."""
         cls, reg, anchors = self._raw_predictions(images)
-        out = []
-        for i in range(images.shape[0]):
-            found = _ops.detect_image0(cls, reg, anchors, images.shape[2], images.shape[3], self.threshold,
-                                       self.iou_threshold, index=i)
-            if found is None:
-                found = [cls.new_zeros(0), torch.zeros(0, dtype=torch.int64, device=cls.device),
-                         cls.new_zeros(0, 4)]
-            out.append(found)
-        return out
+        return _ops.detect_batch(cls, reg, anchors, images.shape[2], images.shape[3], self.threshold,
+                                 self.iou_threshold)
 
     def forward(self, inputs):
         if self.is_training:

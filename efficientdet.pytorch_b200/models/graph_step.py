@@ -1,4 +1,5 @@
-"""CUDA-graph execution of the training step (forward + FocalLoss + backward, optionally the fused optimizer).
+"""CUDA-graph execution of the training step (forward + FocalLoss + backward, optionally the fused optimizer), and of
+inference (GraphedDetect, at the end of this file).
 
 Every kernel of the hot path is launched on the caller's stream with device-resident arguments and no host
 synchronisation (the C ABI never syncs, FocalLoss reads its upstream gradients from device memory), so the ~480
@@ -92,3 +93,83 @@ class GraphedTrainStep:
         self.static_annots.copy_(annotations, non_blocking=True)
         self.graph.replay()
         return self.static_loss
+
+
+class GraphedDetect:
+    """CUDA-graph execution of inference: network forward + decode + threshold + NMS of a whole batch as one replay,
+    with no host synchronisation.
+
+        det = GraphedDetect(model, example_images, max_candidates=8192)   # model.eval(), model.is_training False
+        out = det(images)        # copies into the static input, one replay -> _ops.Detections (padded, on the device)
+        dets = det.to_list(out)  # one device->host read -> B triples exactly as model.detect_batch(images) returns them
+
+    out.scores [B,C], out.classes [B,C] int64, out.boxes [B,C,4] and out.count [B] int32 (kept rows; -1 when the image
+    has more than C candidates above the threshold) are static tensors: every call rewrites them.  C is max_candidates,
+    or the anchor count A when that is smaller (an image never has more than A candidates).  to_list redoes overflowed
+    images eagerly from the network outputs of the last replay.  Calls take images of the example's shape only.
+
+    Memory that max_candidates costs per image: the NMS mask C * ceil(C/64) * 8 bytes (8 MiB at C = 8192) plus
+    32 bytes per row of keep indices and padded outputs.  The decoded anchors and their sort keys (24 bytes per anchor
+    plus 8 per power-of-two padded anchor) do not depend on C.
+
+    The packed weights and folded BatchNorm are derived inside the graph, so replays follow in-place weight updates
+    (load_state_dict, EMA copies).  The score and IoU thresholds are fixed at capture."""
+
+    def __init__(self, model, images, max_candidates=8192, warmup=2):
+        if model.training or model.is_training:
+            raise _ops.N.EffdetNativeError('GraphedDetect needs a model in inference mode (model.eval() and '
+                                           'model.is_training = False)')
+        if not images.is_cuda:
+            raise _ops.N.EffdetNativeError('GraphedDetect needs CUDA example images')
+        self.model = model
+        self.max_candidates = int(max_candidates)
+        self.threshold, self.iou_threshold = model.threshold, model.iou_threshold
+        self.static_images = images.clone()
+        dev = images.device
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(warmup):                                   # anchor table, allocator pools, smem opt-ins
+                self._run()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        _ops.invalidate_caches()                                      # capture the weight packing and BN folding
+        self.graph = torch.cuda.CUDAGraph()
+        n0 = _ops.N.launch_count()
+        with torch.cuda.graph(self.graph):
+            self.cls, self.reg, self.anchors, self.out = self._run()
+        self.library_launches = _ops.N.launch_count() - n0            # kernels of this library recorded into the graph
+        # capture recorded the weight packing without running it: the cache entries it made hold nothing until a
+        # replay.  Dropping them makes eager calls derive their own; the graph keeps its copies in its private pool.
+        _ops.invalidate_caches()
+
+    @torch.no_grad()
+    def _run(self):
+        cls, reg, anchors = self.model._raw_predictions(self.static_images)
+        out = _ops.detect_batch(cls, reg, anchors, self.static_images.shape[2], self.static_images.shape[3],
+                                self.threshold, self.iou_threshold, cap=min(self.max_candidates, cls.shape[1]))
+        return cls, reg, anchors, out
+
+    def __call__(self, images):
+        if (self.model.threshold, self.model.iou_threshold) != (self.threshold, self.iou_threshold):
+            raise _ops.N.EffdetNativeError(
+                'GraphedDetect: threshold / iou_threshold changed from (%r, %r) at capture to (%r, %r); build a new '
+                'GraphedDetect' % (self.threshold, self.iou_threshold, self.model.threshold, self.model.iou_threshold))
+        if images.shape != self.static_images.shape:
+            raise _ops.N.EffdetNativeError('GraphedDetect was captured for images of shape %s, got %s'
+                                           % (tuple(self.static_images.shape), tuple(images.shape)))
+        self.static_images.copy_(images, non_blocking=True)
+        self.graph.replay()
+        return self.out
+
+    def to_list(self, out):
+        """out (the result of the latest call) -> list of B triples [scores[K_b], classes[K_b] int64, boxes[K_b,4]]"""
+        res = []
+        for b, m in enumerate(out.count.tolist()):                   # the one device->host read
+            if m < 0:
+                res.append(_ops.detect_batch(self.cls[b:b + 1], self.reg[b:b + 1], self.anchors,
+                                             self.static_images.shape[2], self.static_images.shape[3], self.threshold,
+                                             self.iou_threshold)[0])
+            else:
+                res.append([out.scores[b, :m], out.classes[b, :m], out.boxes[b, :m]])
+        return res

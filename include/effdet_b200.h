@@ -354,6 +354,33 @@ int effdet_gather_detections(const float* boxes, const float* scores, const int3
                              float* out_boxes, int device, effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * The same post-processing for a batch of B images in one set of launches.  The per-image counts
+ * stay in device memory and no launch's grid depends on them, so the three calls can be
+ * captured in a CUDA graph.  The single-image entry points above run these kernels with B = 1.
+ *   cls [B,A,K], reg [B,A,4] (16-byte aligned), anchors [A,4] shared by all images (16-byte aligned)
+ *   boxes [B,A,4] (16-byte aligned), scores [B,A], classes [B,A] int32: every anchor, decoded and clipped
+ *   keys [B,npad] (npad = pow2 >= A): image b's segment sorted ascending, so that entry j < count[b]
+ *        is its j-th best candidate (score desc, anchor index asc); the rest are ~0 sentinels
+ *   count [B] int32: candidates of image b above the threshold
+ * ------------------------------------------------------------------------------------------ */
+int effdet_detect_candidates_batch(const float* cls, const float* reg, const float* anchors, float* boxes, float* scores,
+                                   int32_t* classes, uint64_t* keys, int32_t* count, int B, int A, int K, int npad,
+                                   float img_w, float img_h, float threshold, int device, effdet_stream_t stream);
+/* Greedy NMS of at most `cap` candidates per image (1 <= cap <= A, ceil(cap/64)*8 <= 200 KiB of scan bitmap).
+ *   boxes [B,A,4], keys [B,npad] and count [B] as written by effdet_detect_candidates_batch
+ *   mask_ws [B][cap][ceil(cap/64)] uint64 workspace
+ *   keep_idx [B][cap] int32: anchor indices of image b's kept boxes, best first, in its first nkeep[b] entries
+ *   nkeep [B] int32: boxes kept in image b, or -1 when count[b] > cap (overflow: nothing else is written for it) */
+int effdet_nms_batch(const float* boxes, const uint64_t* keys, const int32_t* count, int B, int A, int npad, int cap,
+                     double iou_threshold, uint64_t* mask_ws, int32_t* keep_idx, int32_t* nkeep, int device,
+                     effdet_stream_t stream);
+/* Padded detections: row i < nkeep[b] of image b is its i-th kept box, every later row is zero (all rows when
+ * nkeep[b] == -1).  out_scores [B][cap] float, out_classes [B][cap] int64, out_boxes [B][cap][4] float (16-byte aligned). */
+int effdet_gather_detections_batch(const float* boxes, const float* scores, const int32_t* classes,
+                                   const int32_t* keep_idx, const int32_t* nkeep, int B, int A, int cap, float* out_scores,
+                                   int64_t* out_classes, float* out_boxes, int device, effdet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) rank 1: the optimizer step that follows backward in the reference loop,
  *   clip_grad_norm_(parameters, max_norm) + AdamW.step()        (train.py:115-118, train.py:268)
  * as two multi-tensor launches.  The tables live in DEVICE memory: per tensor t its fp32 data pointers and
