@@ -21,7 +21,7 @@ void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memo
 
 }  // namespace effdet
 
-extern "C" int effdet_version(void) { return 100; }
+extern "C" int effdet_version(void) { return 101; }
 extern "C" const char* effdet_last_error(void) { return effdet::err_buf(); }
 extern "C" uint64_t effdet_launch_count(void) { return effdet::g_launches.load(std::memory_order_relaxed); }
 extern "C" void effdet_reset_launch_count(void) { effdet::g_launches.store(0, std::memory_order_relaxed); }

@@ -411,17 +411,8 @@ extern "C" int effdet_conv2d(const effdet_conv_args* a, int device, effdet_strea
     return launch_status("conv_igemm_kernel");
 }
 
-namespace effdet {
-int colsum_launch(const float* x, float* out, long long M, int N, long long HW, long long bstride, int device,
-                  effdet_stream_t stream);
-}
-
-extern "C" int effdet_colsum(const float* x, float* out, int64_t M, int N, int device, effdet_stream_t stream) {
-    return colsum_launch(x, out, M, N, M, 0, device, stream);
-}
-
-int effdet::colsum_launch(const float* x, float* out, long long M, int N, long long HW, long long bstride, int device,
-                          effdet_stream_t stream) {
+static int colsum_launch(const float* x, float* out, long long M, int N, long long HW, long long bstride, int device,
+                         effdet_stream_t stream) {
     EFFDET_REQUIRE(x && out && M > 0 && N > 0 && N % 4 == 0, "colsum: bad arguments");
     EFFDET_REQUIRE(aligned16(x), "colsum: x must be 16-byte aligned");
     EFFDET_DEVICE(device);

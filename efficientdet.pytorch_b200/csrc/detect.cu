@@ -1,7 +1,7 @@
 // Inference post-processing on the device: box decode + clip + per-anchor class max + score
 // threshold + sort + greedy NMS, for a batch of B images.  Every stage covers the whole batch in
 // one set of launches, and the per-image counts stay in device memory, so the launches can be
-// captured in a CUDA graph.  The single-image entry points run the same kernels with B = 1.
+// captured in a CUDA graph.
 // Reference: models/module.py:24-49 (BBoxTransform), :57-67 (ClipBoxes),
 //            models/efficientdet.py:70-86 (threshold, nms, gather), torchvision.ops.nms.
 // Bit-exactness rules (the keep-set must equal torchvision's): fp32 IoU from separately rounded
@@ -138,9 +138,9 @@ __device__ __forceinline__ bool iou_gt(const float4 a, const float4 b, double th
     return (double)ovr > thr;
 }
 
-// Candidates NMS works on in image b: count[b] (all `cap` when count is NULL), or 0 when count[b] > cap (overflow).
+// Candidates NMS works on in image b: count[b], or 0 when count[b] > cap (overflow).
 __device__ __forceinline__ int nms_candidates(const int32_t* count, int b, int cap) {
-    const int n = count ? count[b] : cap;
+    const int n = count[b];
     return n > cap ? 0 : n;
 }
 
@@ -209,7 +209,7 @@ __global__ void __launch_bounds__(1024) nms_scan_kernel(const uint64_t* __restri
     extern __shared__ uint64_t removed[];
     __shared__ uint64_t keep_bits;
     const int b = blockIdx.x;
-    const int n = count ? count[b] : cap;
+    const int n = count[b];
     if (n > cap) {
         if (threadIdx.x == 0) nkeep[b] = -1;
         return;
@@ -259,7 +259,7 @@ __global__ void __launch_bounds__(1024) nms_scan_kernel(const uint64_t* __restri
     if (threadIdx.x == 0) nkeep[b] = kept;
 }
 
-// row i of image b (blockIdx.y): the i-th kept detection, zero from nkeep[b] on (all `cap` rows kept when nkeep is NULL)
+// row i of image b (blockIdx.y): the i-th kept detection, zero from nkeep[b] on
 __global__ void gather_detections_kernel(const float* __restrict__ boxes, const float* __restrict__ scores,
                                          const int32_t* __restrict__ classes, const int32_t* __restrict__ keep_idx,
                                          const int32_t* __restrict__ nkeep, int A, int cap, float* __restrict__ out_scores,
@@ -268,8 +268,7 @@ __global__ void gather_detections_kernel(const float* __restrict__ boxes, const 
     const long long b = blockIdx.y;
     if (i >= cap) return;
     const long long o = b * cap + i;
-    const int m = nkeep ? nkeep[b] : cap;
-    if (i < m) {
+    if (i < nkeep[b]) {
         const long long a = b * A + keep_idx[o];
         out_scores[o] = scores[a];
         out_classes[o] = (long long)classes[a];
@@ -338,37 +337,6 @@ static int gather_launch(const float* boxes, const float* scores, const int32_t*
 }  // namespace effdet
 
 using namespace effdet;
-
-extern "C" int effdet_detect_candidates(const float* cls, const float* reg, const float* anchors, float* boxes,
-                                        float* scores, int32_t* classes, uint64_t* keys, int32_t* count, int A, int K,
-                                        int npad, float img_w, float img_h, float threshold, int device,
-                                        effdet_stream_t stream) {
-    EFFDET_REQUIRE(cls && reg && anchors && boxes && scores && classes && keys && count, "detect_candidates: null tensor");
-    EFFDET_REQUIRE(A > 0 && K > 0 && npad >= A && (npad & (npad - 1)) == 0, "detect_candidates: npad must be a power of two >= A");
-    EFFDET_REQUIRE(aligned16(reg) && aligned16(anchors) && aligned16(boxes), "detect_candidates: alignment");
-    EFFDET_DEVICE(device);
-    return candidates_launch(cls, reg, anchors, boxes, scores, classes, keys, count, 1, A, K, npad, img_w, img_h, threshold,
-                             (cudaStream_t)stream);
-}
-
-extern "C" int effdet_nms(const float* boxes, const uint64_t* keys, int n, double iou_threshold, uint64_t* mask_ws,
-                          int32_t* keep_idx, int32_t* nkeep, int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(boxes && keys && mask_ws && keep_idx && nkeep && n > 0, "nms: bad arguments");
-    EFFDET_REQUIRE((size_t)cdiv(n, 64) * sizeof(uint64_t) <= kScanSmemLimit, "nms: too many candidates for the scan bitmap (%d)", n);
-    EFFDET_DEVICE(device);
-    return nms_launch(boxes, keys, nullptr, 1, 0, 0, n, iou_threshold, mask_ws, keep_idx, nkeep, (cudaStream_t)stream);
-}
-
-extern "C" int effdet_gather_detections(const float* boxes, const float* scores, const int32_t* classes,
-                                        const int32_t* keep_idx, int nkeep, float* out_scores, int64_t* out_classes,
-                                        float* out_boxes, int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(boxes && scores && classes && keep_idx && out_scores && out_classes && out_boxes && nkeep > 0,
-                   "gather_detections: bad arguments");
-    EFFDET_REQUIRE(aligned16(boxes) && aligned16(out_boxes), "gather_detections: alignment");
-    EFFDET_DEVICE(device);
-    return gather_launch(boxes, scores, classes, keep_idx, nullptr, 1, 0, nkeep, out_scores, out_classes, out_boxes,
-                         (cudaStream_t)stream);
-}
 
 extern "C" int effdet_detect_candidates_batch(const float* cls, const float* reg, const float* anchors, float* boxes,
                                               float* scores, int32_t* classes, uint64_t* keys, int32_t* count, int B, int A,

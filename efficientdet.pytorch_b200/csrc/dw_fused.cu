@@ -410,6 +410,13 @@ static int pick_tiles_per_cta(long long ntiles, long long other) {
     return (int)tpc;
 }
 
+__global__ void pack_dw_weight_kernel(const float* __restrict__ w, float* __restrict__ o, int C, int kk) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;  // output index [tap][c]
+    if (i >= C * kk) return;
+    const int c = i % C, tap = i / C;
+    o[i] = __ldg(w + c * kk + tap);
+}
+
 }  // namespace effdet
 
 using namespace effdet;
@@ -509,4 +516,12 @@ extern "C" int effdet_dwconv_bwd_fused(const effdet_dw_bwd_args* a, int device, 
 #undef EFFDET_DWB_KS
 #undef EFFDET_DWB
     return launch_status("dw_bwd_fused_kernel");
+}
+
+extern "C" int effdet_pack_dw_weight(const float* w_c1kk, float* w_kkc, int C, int k, int device,
+                                     effdet_stream_t stream) {
+    EFFDET_REQUIRE(w_c1kk && w_kkc && C > 0 && (k == 3 || k == 5), "pack_dw_weight: bad arguments");
+    EFFDET_DEVICE(device);
+    pack_dw_weight_kernel<<<cdiv((long long)C * k * k, 256), 256, 0, (cudaStream_t)stream>>>(w_c1kk, w_kkc, C, k * k);
+    return launch_status("pack_dw_weight_kernel");
 }

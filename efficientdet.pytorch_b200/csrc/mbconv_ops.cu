@@ -72,12 +72,12 @@ __global__ void __launch_bounds__(256) bnact_bwd_kernel(const effdet_bnact_bwd_a
     }
 }
 
-// out[b,c] += alpha * sum_r a[b,r,c] * (b2 ? b2[b,r,c] : 1);  with scale/shift, b2 is a raw conv output and the factor
-// is swish(b2*scale+shift) (the activated tensor is recomputed instead of stored)
-__global__ void __launch_bounds__(256) spatial_reduce_kernel(const float* __restrict__ a, const float* __restrict__ b2,
+// out[b,c] += alpha * sum_r a[b,r,c] * swish(z[b,r,c]*scale[c]+shift[c]): z is the raw conv output, and the activated
+// tensor is recomputed instead of stored
+__global__ void __launch_bounds__(256) spatial_reduce_kernel(const float* __restrict__ a, const float* __restrict__ z,
                                                              float* __restrict__ out, float alpha, int HW, int C,
-                                                             int rows_per_block, const float* __restrict__ scale = nullptr,
-                                                             const float* __restrict__ shift = nullptr) {
+                                                             int rows_per_block, const float* __restrict__ scale,
+                                                             const float* __restrict__ shift) {
     __shared__ float4 red[256];
     const int cvecs = C / 4;
     const RowPack rp = rowpack(cvecs, blockIdx.y);
@@ -86,27 +86,22 @@ __global__ void __launch_bounds__(256) spatial_reduce_kernel(const float* __rest
     if (rp.active) {
         const int r_begin = blockIdx.x * rows_per_block;
         const int r_end = min(HW, r_begin + rows_per_block);
-        float4 sc = f4zero(), sh = f4zero();
-        if (scale) { sc = ldg4(scale + rp.cv * 4); sh = ldg4(shift + rp.cv * 4); }
+        const float4 sc = ldg4(scale + rp.cv * 4), sh = ldg4(shift + rp.cv * 4);
         constexpr int U = 4;                            // 8 independent 128-bit loads in flight per thread
         for (int r0 = r_begin + rp.tr; r0 < r_end; r0 += U * rp.rows) {
-            float4 av[U], bv[U];
+            float4 av[U], zv[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) {
                 const int r = r0 + u * rp.rows;
                 const long long off = ((long long)b * HW + (r < r_end ? r : r0)) * C + rp.cv * 4;
                 av[u] = ldg4(a + off);
-                bv[u] = b2 ? ldg4(b2 + off) : make_float4(1.f, 1.f, 1.f, 1.f);
+                zv[u] = ldg4(z + off);
             }
 #pragma unroll
             for (int u = 0; u < U; ++u) {
                 if (r0 + u * rp.rows >= r_end) break;
-                float4 w = bv[u];
-                if (scale) {
-                    const float4 q = f4fma(w, sc, sh);
-                    w = make_float4(swishf_(q.x), swishf_(q.y), swishf_(q.z), swishf_(q.w));
-                }
-                s = f4fma(av[u], w, s);
+                const float4 q = f4fma(zv[u], sc, sh);
+                s = f4fma(av[u], make_float4(swishf_(q.x), swishf_(q.y), swishf_(q.z), swishf_(q.w)), s);
             }
         }
     }
@@ -209,18 +204,6 @@ extern "C" int effdet_bnact_bwd(const effdet_bnact_bwd_args* a, int device, effd
     row_grid(a->HW, a->C / 4, a->B, &grid, &rpb);
     bnact_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(*a, rpb);
     return launch_status("bnact_bwd_kernel");
-}
-
-extern "C" int effdet_spatial_reduce(const float* a, const float* b2, float* out, float alpha, int B, int HW, int C,
-                                     int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(a && out && B > 0 && B <= 65535 && HW > 0 && C > 0 && C % 4 == 0, "spatial_reduce: bad arguments");
-    EFFDET_REQUIRE(aligned16(a) && aligned16(b2), "spatial_reduce: alignment");
-    EFFDET_DEVICE(device);
-    dim3 grid;
-    int rpb;
-    row_grid(HW, C / 4, B, &grid, &rpb);
-    spatial_reduce_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a, b2, out, alpha, HW, C, rpb);
-    return launch_status("spatial_reduce_kernel");
 }
 
 extern "C" int effdet_spatial_reduce_act(const float* a, const float* z, const float* scale, const float* shift, float* out,

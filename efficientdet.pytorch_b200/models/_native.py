@@ -14,7 +14,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.normpath(os.path.join(_HERE, '..', 'csrc'))
 SO_PATH = os.path.join(CSRC, 'libeffdet_b200.so')
-SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_planes.cu', 'pw_gemm.cu', 'pw_wgrad.cu', 'stem.cu', 'depthwise.cu', 'dw_fused.cu', 'mbconv_ops.cu', 'se_ops.cu', 'bifpn.cu', 'pipeline.cu',
+SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_planes.cu', 'pw_gemm.cu', 'pw_wgrad.cu', 'stem.cu', 'dw_fused.cu', 'mbconv_ops.cu', 'se_ops.cu', 'bifpn.cu', 'pipeline.cu',
            'loss.cu', 'detect.cu', 'layout.cu', 'optim.cu']
 NVCC_FLAGS = ['-std=c++17', '-O3', '-lineinfo', '-gencode', 'arch=compute_90a,code=sm_90a',
               '-Xcompiler', '-fPIC', '-shared']
@@ -137,12 +137,8 @@ SIGNATURES = {
     'effdet_conv2d_wgrad_multi': [ctypes.POINTER(WgradArgs), _INT] + _TAIL,
     'effdet_pack_conv_weight': [_P, _P, _P, _INT, _INT, _INT] + _TAIL,
     'effdet_pack_conv_weight_tc': [_P, _P, _P, _INT, _INT, _INT] + _TAIL,
-    'effdet_colsum': [_P, _P, _I64, _INT] + _TAIL,
     'effdet_stem_fwd': [_P, _P, _P, _P, _P, _P, _INT, _INT, _INT, _INT] + _TAIL,
     'effdet_stem_wgrad': [_P, _P, _P, _INT, _INT, _INT, _INT] + _TAIL,
-    'effdet_dwconv_fwd': [_P, _P, _P, _P, _P, _P] + [_INT] * 10 + _TAIL,
-    'effdet_dwconv_bwd_data': [_P, _P, _P] + [_INT] * 10 + _TAIL,
-    'effdet_dwconv_bwd_weight': [_P, _P, _P] + [_INT] * 10 + _TAIL,
     'effdet_pack_dw_weight': [_P, _P, _INT, _INT] + _TAIL,
     'effdet_dwconv_fwd_fused': [ctypes.POINTER(DwFwdArgs)] + _TAIL,
     'effdet_dwconv_bwd_fused': [ctypes.POINTER(DwBwdArgs)] + _TAIL,
@@ -150,7 +146,6 @@ SIGNATURES = {
     'effdet_bn_fold': [_P, _P, _P, _P, _F, _P, _P, _P, _INT] + _TAIL,
     'effdet_add': [_P, _P, _P, _I64] + _TAIL,
     'effdet_relu_bwd': [_P, _P, _P, _I64] + _TAIL,
-    'effdet_spatial_reduce': [_P, _P, _P, _F, _INT, _INT, _INT] + _TAIL,
     'effdet_spatial_reduce_act': [_P, _P, _P, _P, _P, _F, _INT, _INT, _INT] + _TAIL,
     'effdet_se_gate_fwd': [_P] * 7 + [_INT] * 3 + _TAIL,
     'effdet_se_gate_bwd': [_P] * 12 + [_INT] * 3 + _TAIL,
@@ -159,9 +154,6 @@ SIGNATURES = {
     'effdet_focal_loss_fwd': [_P] * 7 + [_INT] * 4 + [_F, _F] + _TAIL,
     'effdet_focal_loss_bwd': [_P] * 9 + [_INT] * 4 + [_F, _F] + _TAIL,
     'effdet_sigmoid_bwd': [_P, _P, _P, _I64] + _TAIL,
-    'effdet_detect_candidates': [_P] * 8 + [_INT, _INT, _INT, _F, _F, _F] + _TAIL,
-    'effdet_nms': [_P, _P, _INT, ctypes.c_double, _P, _P, _P] + _TAIL,
-    'effdet_gather_detections': [_P, _P, _P, _P, _INT, _P, _P, _P] + _TAIL,
     'effdet_detect_candidates_batch': [_P] * 8 + [_INT, _INT, _INT, _INT, _F, _F, _F] + _TAIL,
     'effdet_nms_batch': [_P, _P, _P, _INT, _INT, _INT, _INT, ctypes.c_double, _P, _P, _P] + _TAIL,
     'effdet_gather_detections_batch': [_P, _P, _P, _P, _P, _INT, _INT, _INT, _P, _P, _P] + _TAIL,

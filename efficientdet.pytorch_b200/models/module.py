@@ -142,7 +142,7 @@ class Anchors(nn.Module):
 
 class BBoxTransform(nn.Module):
     """Box decoding constants (std, mean); the arithmetic is fused with clipping / class-max / threshold
-    in ``effdet_detect_candidates`` (reference models/module.py:24-49)."""
+    in ``effdet_detect_candidates_batch`` (reference models/module.py:24-49)."""
 
     def __init__(self, mean=None, std=None):
         super().__init__()

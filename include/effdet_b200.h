@@ -167,9 +167,6 @@ int effdet_wgrad_tc_geometry_ok(int B, int H, int W);
 int effdet_pack_conv_weight_tc(const float* w_oihw, void* w_fwd, void* w_dgrad, int Cout, int Cin, int ksize,
                                int device, effdet_stream_t stream);
 
-/* out[n] += sum_m x[m,n]   (bias gradients, BN beta gradients) */
-int effdet_colsum(const float* x, float* out, int64_t M, int N, int device, effdet_stream_t stream);
-
 /* ------------------------------------------------------------------------------------------
  * Stem: 3x3 stride-2 conv on the NCHW image with TF-"SAME" pad (0,1,0,1), eval-BN, swish.
  * Replaces EfficientNet.extract_features stem, models/efficientnet.py:193 (+ utils.py:126-155).
@@ -183,23 +180,9 @@ int effdet_stem_wgrad(const float* x_nchw, const float* dz, float* dw_oihw, int 
                       int device, effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Depthwise k x k (k in {3,5}), stride in {1,2}, asymmetric TF-"SAME" pad, eval-BN, swish.
- * Replaces MBConvBlock.forward depthwise phase, models/efficientnet.py:87.
- *   x [B,H,W,C] -> z raw, y = swish(z*scale+shift), both [B,Ho,Wo,C];  w_kkc = [k][k][C]
- * ------------------------------------------------------------------------------------------ */
-int effdet_dwconv_fwd(const float* x, const float* w_kkc, const float* scale, const float* shift, float* z, float* y,
-                      int B, int H, int W, int C, int k, int stride, int pad_t, int pad_l, int Ho, int Wo,
-                      int device, effdet_stream_t stream);
-int effdet_dwconv_bwd_data(const float* dz, const float* w_kkc, float* dx, int B, int H, int W, int C, int k,
-                           int stride, int pad_t, int pad_l, int Ho, int Wo, int device, effdet_stream_t stream);
-/* dw[C,1,k,k] += ... */
-int effdet_dwconv_bwd_weight(const float* x, const float* dz, float* dw_c1kk, int B, int H, int W, int C, int k,
-                             int stride, int pad_t, int pad_l, int Ho, int Wo, int device, effdet_stream_t stream);
-int effdet_pack_dw_weight(const float* w_c1kk, float* w_kkc, int C, int k, int device, effdet_stream_t stream);
-
-/* ------------------------------------------------------------------------------------------
  * Depthwise phase of MBConvBlock.forward with only PRE-activations in HBM (the reference's
  * MemoryEfficientSwish saves the pre-activation only, models/utils.py:31-42; block: models/efficientnet.py:85-94).
+ * Depthwise k x k (k in {3,5}), stride in {1,2}, w_kkc = [k][k][C] (effdet_pack_dw_weight).
  * Pads must be the reference's static ones (models/utils.py:126-149): k3s1 1, k5s1 2, k3s2 0, k5s2 1 (top/left).
  *   fwd: a0 = in_scale ? swish(x*in_scale+in_shift) : x        (BN0+swish applied while the tile is staged)
  *        z  = depthwise(a0)                                    raw output, the only tensor written
@@ -239,6 +222,8 @@ typedef struct {
                               consume directly (effdet_conv_args.x_planes, effdet_wgrad_args.dy_planes); C % 8 == 0 */
 } effdet_dw_bwd_args;
 int effdet_dwconv_bwd_fused(const effdet_dw_bwd_args* a, int device, effdet_stream_t stream);
+/* depthwise weight [C,1,k,k] -> w_kkc [k][k][C] */
+int effdet_pack_dw_weight(const float* w_c1kk, float* w_kkc, int C, int k, int device, effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Backward of  y = act(BN_eval(z)) [* row_scale]  with frozen statistics but trainable affine
@@ -270,15 +255,13 @@ int effdet_relu_bwd(const float* dy, const float* y, float* dz, int64_t n, int d
 
 /* ------------------------------------------------------------------------------------------
  * Squeeze-excite (models/efficientnet.py:90-94).
- *   effdet_spatial_reduce : out[b,c] += alpha * sum_hw a[b,hw,c] * (b2 ? b2[b,hw,c] : 1)
- *   effdet_se_gate_fwd    : s_pre = W1*mean+b1 ; gate = sigmoid(W2*swish(s_pre)+b2)
- *   effdet_se_gate_bwd    : given dgate -> dmean, and += into dW1,db1,dW2,db2
+ *   effdet_spatial_reduce_act : out[b,c] += alpha * sum_hw a[b,hw,c] * swish(z[b,hw,c]*scale[c]+shift[c])
+ *                               (gradient w.r.t. the SE gate from the raw depthwise output: the activated tensor is
+ *                               recomputed, not stored)
+ *   effdet_se_gate_fwd        : s_pre = W1*mean+b1 ; gate = sigmoid(W2*swish(s_pre)+b2)
+ *   effdet_se_gate_bwd        : given dgate -> dmean, and += into dW1,db1,dW2,db2
  * W1 = _se_reduce.weight [S,C], W2 = _se_expand.weight [C,S].
  * ------------------------------------------------------------------------------------------ */
-int effdet_spatial_reduce(const float* a, const float* b2, float* out, float alpha, int B, int HW, int C,
-                          int device, effdet_stream_t stream);
-/*   effdet_spatial_reduce_act : out[b,c] += alpha * sum_hw a[b,hw,c] * swish(z[b,hw,c]*scale[c]+shift[c])
- *   (gradient w.r.t. the SE gate from the raw depthwise output: the activated tensor is recomputed, not stored) */
 int effdet_spatial_reduce_act(const float* a, const float* z, const float* scale, const float* shift, float* out,
                               float alpha, int B, int HW, int C, int device, effdet_stream_t stream);
 int effdet_se_gate_fwd(const float* mean, const float* w1, const float* b1, const float* w2, const float* b2,
@@ -336,27 +319,10 @@ int effdet_focal_loss_bwd(const float* cls, const float* reg, const float* ancho
 /* y = g * p*(1-p) (sigmoid backward) ; y may alias g */
 int effdet_sigmoid_bwd(const float* g, const float* p, float* y, int64_t n, int device, effdet_stream_t stream);
 /* ------------------------------------------------------------------------------------------
- * Inference post-processing of image 0 (models/efficientdet.py:70-86, models/module.py:24-67,
- * torchvision.ops.nms): decode + clip + class max + threshold + sort + greedy NMS, all on the
- * device; the host only reads the two counters to size its output tensors.
- * ------------------------------------------------------------------------------------------ */
-/* boxes[A,4], scores[A], classes[A]; keys[npad] (npad = pow2 >= A) sorted ascending so that
- * entry j < *count is the j-th best candidate (score desc, anchor index asc); count[0] = #cands. */
-int effdet_detect_candidates(const float* cls, const float* reg, const float* anchors, float* boxes, float* scores,
-                             int32_t* classes, uint64_t* keys, int32_t* count, int A, int K, int npad,
-                             float img_w, float img_h, float threshold, int device, effdet_stream_t stream);
-/* mask_ws: n * ceil(n/64) uint64; keep_idx[n] int32 (anchor indices, best first); nkeep[0] */
-int effdet_nms(const float* boxes, const uint64_t* keys, int n, double iou_threshold, uint64_t* mask_ws,
-               int32_t* keep_idx, int32_t* nkeep, int device, effdet_stream_t stream);
-/* gathers scores/classes(int64)/boxes rows listed in keep_idx */
-int effdet_gather_detections(const float* boxes, const float* scores, const int32_t* classes,
-                             const int32_t* keep_idx, int nkeep, float* out_scores, int64_t* out_classes,
-                             float* out_boxes, int device, effdet_stream_t stream);
-
-/* ------------------------------------------------------------------------------------------
- * The same post-processing for a batch of B images in one set of launches.  The per-image counts
- * stay in device memory and no launch's grid depends on them, so the three calls can be
- * captured in a CUDA graph.  The single-image entry points above run these kernels with B = 1.
+ * Inference post-processing (models/efficientdet.py:70-86, models/module.py:24-67, torchvision.ops.nms):
+ * decode + clip + class max + threshold + sort + greedy NMS for a batch of B images in one set of
+ * launches, all on the device.  The per-image counts stay in device memory and no launch's grid
+ * depends on them, so the three calls can be captured in a CUDA graph.
  *   cls [B,A,K], reg [B,A,4] (16-byte aligned), anchors [A,4] shared by all images (16-byte aligned)
  *   boxes [B,A,4] (16-byte aligned), scores [B,A], classes [B,A] int32: every anchor, decoded and clipped
  *   keys [B,npad] (npad = pow2 >= A): image b's segment sorted ascending, so that entry j < count[b]

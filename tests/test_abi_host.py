@@ -65,7 +65,7 @@ def test_ctypes_struct_layout_matches_header(native, tmp_path):
             assert int(out['%s.%s' % (cname, fname)]) == getattr(cls, fname).offset, (cname, fname)
 
 
-def test_argument_validation_and_error_plumbing(native):
+def test_argument_refusals_and_error_plumbing(native):
     """the boundary's error behaviour (include/effdet_b200.h): arguments are validated BEFORE anything touches the
     device, a failing call returns a negative code and leaves its reason in the thread-local effdet_last_error();
     these calls never reach a kernel launch, so they run without a GPU"""
@@ -78,14 +78,15 @@ def test_argument_validation_and_error_plumbing(native):
     fake = 1 << 20                                           # aligned non-null "pointer"; never dereferenced
     assert lib.effdet_conv2d(None, 0, None) == -1 and 'null' in err()
     assert lib.effdet_conv2d(ctypes.byref(native.ConvArgs()), 0, None) == -1 and 'null' in err()
-    assert lib.effdet_dwconv_fwd(fake, fake, fake, fake, fake, fake, 1, 8, 8, 8, 4, 1, 1, 1, 8, 8, 0, None) == -1
-    assert 'k=4' in err()
-    assert lib.effdet_dwconv_fwd(fake, fake, fake, fake, fake, fake, 1, 8, 8, 6, 3, 1, 1, 1, 8, 8, 0, None) == -1
-    assert 'multiple of 4' in err()
+    dw = native.DwFwdArgs(x=fake, w_kkc=fake, scale=fake, shift=fake, z=fake, se_sum=fake,
+                          B=1, H=8, W=8, C=8, k=4, stride=1, pad_t=1, pad_l=1, Ho=8, Wo=8)
+    assert lib.effdet_dwconv_fwd_fused(ctypes.byref(dw), 0, None) == -1 and 'k=4' in err()
+    dw.C, dw.k = 6, 3
+    assert lib.effdet_dwconv_fwd_fused(ctypes.byref(dw), 0, None) == -1 and 'multiple of 4' in err()
     assert lib.effdet_focal_loss_fwd(fake, fake, fake, fake, fake, fake, fake, 1, 100, 20, 1000, 0.25, 2.0, 0, None) == -1
     assert 'G=1000' in err() and '256' in err()
     assert lib.effdet_stem_fwd(fake, fake, fake, fake, fake, fake, 1, 512, 512, 30, 0, None) == -1 and 'C0=30' in err()
-    assert lib.effdet_nms(fake, fake, 0, 0.5, fake, fake, fake, 0, None) == -1 and 'nms' in err()
+    assert lib.effdet_nms_batch(fake, fake, fake, 1, 100, 128, 0, 0.5, fake, fake, fake, 0, None) == -1 and 'nms' in err()
     assert lib.effdet_multi_sumsq(None, None, None, None, 0, 0, None, 0, None) == -1 and 'multi_sumsq' in err()
     assert lib.effdet_add(fake + 4, fake, fake, 64, 0, None) == -1 and 'alignment' in err()
     assert lib.effdet_add(fake, fake, fake, 62, 0, None) == -1 and 'multiple of 4' in err()

@@ -121,6 +121,52 @@ def test_nms_batch_keep_sets_equal_torchvision_golden():
 
 
 @gpu
+def test_detect_candidates_sort_and_decode():
+    """B = 2 seeded draws, each with a block of exactly tied scores above the threshold: per image, scores and classes
+    equal the oracle's class max, boxes its decode + clip, and the sorted key segment (sentinels included) equals the
+    host keys, so candidates come best first with ties broken by anchor index"""
+    from models import _native as N
+    A, K, npad, thr = 5000, 20, 8192, 0.93
+    g = torch.Generator().manual_seed(17)
+    cls0 = torch.rand(1, A, K, generator=g)
+    cls0[0, 100:400] = cls0[0, 100:101]                # exact score ties -> index order must decide
+    reg0 = torch.randn(1, A, 4, generator=g) * 0.5
+    xy = torch.rand(A, 2, generator=g) * 200
+    anchors = torch.cat([xy, xy + torch.rand(A, 2, generator=g) * 60 + 4], dim=1)
+    g = torch.Generator().manual_seed(18)
+    cls1 = torch.rand(1, A, K, generator=g)
+    cls1[0, 2000:2600] = cls1[0, 2000:2001]
+    reg1 = torch.randn(1, A, 4, generator=g) * 0.5
+    cls, reg = torch.cat([cls0, cls1]), torch.cat([reg0, reg1])
+    B, ties = 2, (slice(100, 400), slice(2000, 2600))
+    d = _dev()
+    boxes = torch.empty(B, A, 4, device=d); scores = torch.empty(B, A, device=d)
+    classes = torch.empty(B, A, dtype=torch.int32, device=d); keys = torch.empty(B, npad, dtype=torch.int64, device=d)
+    count = torch.empty(B, dtype=torch.int32, device=d)
+    cd, rd, ad = cls.to(d), reg.to(d), anchors.to(d)
+    N.call('effdet_detect_candidates_batch', cd, N.f32(cd), N.f32(rd), N.f32(ad), N.f32(boxes), N.f32(scores),
+           classes.data_ptr(), keys.data_ptr(), count.data_ptr(), B, A, K, npad, 256.0, 224.0, thr)
+    ref_boxes = O.clip_boxes(O.decode_boxes(anchors[None], reg), 224, 256)
+    for b in range(B):
+        ref_s, ref_c = cls[b].max(dim=1)
+        assert torch.equal(scores[b].cpu(), ref_s), b
+        assert torch.equal(classes[b].cpu().long(), ref_c), b
+        assert O.rel_err(boxes[b].cpu(), ref_boxes[b]) < 1e-6, b
+        mask = ref_s > thr
+        assert bool(mask[ties[b]].all()) and ref_s[ties[b]].unique().numel() == 1, b
+        n = int(mask.sum())
+        assert int(count[b]) == n and n > 100, b
+        hk = _host_keys(ref_s.numpy())
+        hk[~mask.numpy()] = np.uint64(0xffffffffffffffff)
+        full = np.full(npad, np.uint64(0xffffffffffffffff), dtype=np.uint64)
+        full[:A] = hk
+        assert np.array_equal(keys[b].cpu().numpy().view(np.uint64), np.sort(full)), b
+        order = (keys[b, :n].cpu().numpy().view(np.uint64) & np.uint64(0xffffffff)).astype(np.int64)
+        ref_order = torch.nonzero(mask)[:, 0][torch.sort(ref_s[mask], descending=True, stable=True)[1]]
+        assert np.array_equal(order, ref_order.numpy()), b
+
+
+@gpu
 def test_real_model_keep_sets_exact_and_batch_equals_slices():
     """D0 256x256, B = 4, random weights, a threshold passing a few hundred candidates and one image with none: every
     keep-set equals the oracle's greedy NMS over the device's own decoded candidates, and the batched call is

@@ -688,72 +688,6 @@ def test_anchors_bit_exact():
     assert hashlib.sha256(a.tobytes()).digest() == bytes(st['anchors/sha256'])
 
 
-def _host_keys(scores):
-    """sort keys exactly as effdet_detect_candidates builds them: (~order(score)) << 32 | index."""
-    u = scores.astype(np.float32).view(np.uint32).astype(np.uint64)
-    neg = (u & np.uint64(0x80000000)) != 0
-    order = np.where(neg, (~u) & np.uint64(0xffffffff), u | np.uint64(0x80000000))
-    inv = (~order) & np.uint64(0xffffffff)
-    return (inv << np.uint64(32)) | np.arange(scores.shape[0], dtype=np.uint64)
-
-
-def test_nms_keep_set_bit_exact_vs_torchvision_golden():
-    """same boxes/scores as the torchvision goldens -> identical keep indices, order included."""
-    from models import _native as N
-    st = np.load(os.path.join(G, 'nms_torchvision.npz'))
-    for c in range(4):
-        boxes = torch.from_numpy(st['c%d/boxes' % c]).to(_dev())
-        scores = st['c%d/scores' % c]
-        n = boxes.shape[0]
-        keys = torch.from_numpy(np.sort(_host_keys(scores)).view(np.int64)).to(_dev())
-        cb = (n + 63) // 64
-        mask = torch.empty(n * cb, dtype=torch.int64, device=_dev())
-        keep = torch.empty(n, dtype=torch.int32, device=_dev())
-        nkeep = torch.zeros(1, dtype=torch.int32, device=_dev())
-        N.call('effdet_nms', boxes, N.f32(boxes), keys.data_ptr(), n, 0.5, mask.data_ptr(), keep.data_ptr(),
-               nkeep.data_ptr())
-        k = int(nkeep.item())
-        ref = st['c%d/keep' % c]
-        assert k == ref.shape[0], (c, k, ref.shape[0])
-        assert np.array_equal(keep[:k].cpu().numpy().astype(np.int64), ref), c
-
-
-def test_detect_candidates_sort_and_decode():
-    from models import _native as N
-    g = torch.Generator().manual_seed(17)
-    A, K = 5000, 20
-    cls = torch.rand(1, A, K, generator=g)
-    cls[0, 100:400] = cls[0, 100:101]                 # exact score ties -> index order must decide
-    reg = torch.randn(1, A, 4, generator=g) * 0.5
-    xy = torch.rand(A, 2, generator=g) * 200
-    anchors = torch.cat([xy, xy + torch.rand(A, 2, generator=g) * 60 + 4], dim=1)
-    thr = 0.93
-    npad = 8192
-    d = _dev()
-    boxes = torch.empty(A, 4, device=d); scores = torch.empty(A, device=d)
-    classes = torch.empty(A, dtype=torch.int32, device=d); keys = torch.empty(npad, dtype=torch.int64, device=d)
-    count = torch.zeros(1, dtype=torch.int32, device=d)
-    cd, rd, ad = cls[0].contiguous().to(d), reg[0].contiguous().to(d), anchors.to(d)
-    N.call('effdet_detect_candidates', cd, N.f32(cd), N.f32(rd), N.f32(ad), N.f32(boxes), N.f32(scores),
-           classes.data_ptr(), keys.data_ptr(), count.data_ptr(), A, K, npad, 256.0, 224.0, thr)
-    ref_boxes = O.clip_boxes(O.decode_boxes(anchors[None], reg), 224, 256)[0]
-    ref_s, ref_c = cls[0].max(dim=1)
-    assert torch.equal(scores.cpu(), ref_s)
-    assert torch.equal(classes.cpu().long(), ref_c)
-    assert _rel(boxes.cpu(), ref_boxes) < 1e-6
-    mask = ref_s > thr
-    n = int(mask.sum())
-    assert int(count.item()) == n and n > 100
-    hk = _host_keys(ref_s.numpy())
-    hk[~mask.numpy()] = np.uint64(0xffffffffffffffff)
-    full = np.full(npad, np.uint64(0xffffffffffffffff), dtype=np.uint64)
-    full[:A] = hk
-    assert np.array_equal(keys.cpu().numpy().view(np.uint64), np.sort(full))
-    order = (keys[:n].cpu().numpy().view(np.uint64) & np.uint64(0xffffffff)).astype(np.int64)
-    ref_order = torch.nonzero(mask)[:, 0][torch.sort(ref_s[mask], descending=True, stable=True)[1]]
-    assert np.array_equal(order, ref_order.numpy())
-
-
 # ------------------------------------------------------------------------------------------------
 # whole model vs golden vectors of the real reference
 # ------------------------------------------------------------------------------------------------

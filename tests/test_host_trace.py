@@ -126,27 +126,6 @@ class Recorder:
                 self.need(a['in_scale'], a['Cin'], name + ' in_scale'); self.need(a['in_shift'], a['Cin'], name + ' in_shift')
                 assert (a['ws_x'] is None) == (a['precision'] == 0 or a['x_planes'] is not None)
                 assert (a['ws_dy'] is None) == (a['precision'] == 0 or a['dy_planes'] is not None)
-        elif name in ('effdet_dwconv_fwd', 'effdet_dwconv_bwd_data', 'effdet_dwconv_bwd_weight'):
-            B, H, W, C, k, stride, pad_t, pad_l, Ho, Wo = snap[-10:]
-            # Conv2dStaticSamePadding on even maps == TF-SAME (models/utils.py:126-155; SURVEY.md 8(a) row B3)
-            assert (k, stride) in ((3, 1), (3, 2), (5, 1), (5, 2))
-            assert (pad_t, pad_l) == {(3, 1): (1, 1), (3, 2): (0, 0), (5, 1): (2, 2), (5, 2): (1, 1)}[(k, stride)]
-            # the pads are STATIC (computed once for image_size 224), so the output size follows the conv formula,
-            # which equals ceil(H/stride) only on even maps
-            total = {(3, 1): 2, (3, 2): 1, (5, 1): 4, (5, 2): 3}[(k, stride)]
-            assert Ho == (H + total - k) // stride + 1 and Wo == (W + total - k) // stride + 1 and C % 4 == 0
-            big, small = B * H * W * C, B * Ho * Wo * C
-            if name == 'effdet_dwconv_fwd':
-                x, w, scale, shift, z, y = snap[:6]
-                self.need(x, big, 'dw x'); self.need(w, k * k * C, 'dw w')
-                self.need(scale, C, 'dw scale'); self.need(shift, C, 'dw shift')
-                self.need(z, small, 'dw z'); self.need(y, small, 'dw y')
-            elif name == 'effdet_dwconv_bwd_data':
-                dz, w, dx = snap[:3]
-                self.need(dz, small, 'dw dz'); self.need(w, k * k * C, 'dw w'); self.need(dx, big, 'dw dx')
-            else:
-                x, dz, dw = snap[:3]
-                self.need(x, big, 'dw x'); self.need(dz, small, 'dw dz'); self.need(dw, k * k * C, 'dw dw')
         elif name == 'effdet_conv_planes_multi':
             levels = snap[0]
             assert snap[1] == len(levels) and 1 <= len(levels) <= 8
@@ -211,9 +190,6 @@ class Recorder:
             x, dz, dw, B, H, W, C0 = snap
             self.need(x, B * 3 * H * W, 'stem x'); self.need(dz, B * (H // 2) * (W // 2) * C0, 'stem dz')
             self.need(dw, C0 * 27, 'stem dw')
-        elif name == 'effdet_spatial_reduce':
-            a, b2, out, alpha, B, HW, C = snap
-            self.need(a, B * HW * C, 'reduce a'); self.need(b2, B * HW * C, 'reduce b2'); self.need(out, B * C, 'reduce out')
         elif name == 'effdet_se_gate_fwd':
             mean, w1, b1, w2, b2, s_pre, gate, B, C, S = snap
             assert S >= 1
