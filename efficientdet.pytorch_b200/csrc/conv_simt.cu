@@ -10,17 +10,6 @@
 
 namespace effdet {
 
-// tensor-core path (conv_tc.cu)
-bool conv_tc_eligible(const effdet_conv_args* a);
-int conv_tc_launch(const effdet_conv_args* levels, int nlevels, cudaStream_t st);
-bool wgrad_tc_eligible(const effdet_wgrad_args* a);
-bool pw_wgrad_eligible(const effdet_wgrad_args* a);
-int pw_wgrad_launch(const effdet_wgrad_args* a, cudaStream_t st);
-// persistent pointwise GEMM (pw_gemm.cu)
-bool pw_gemm_eligible(const effdet_conv_args* a);
-int pw_gemm_launch(const effdet_conv_args* a, cudaStream_t st);
-int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st, bool* dbias_done);
-
 constexpr int kBM = 128;   // output pixels per CTA
 constexpr int kBK = 16;    // reduction slice (channels of one tap)
 constexpr int kNT = 256;   // threads per CTA
@@ -368,34 +357,8 @@ __global__ void pack_conv_weight_kernel(const float* __restrict__ w, float* __re
     }
 }
 
-}  // namespace effdet
-
-using namespace effdet;
-
-extern "C" int effdet_conv2d(const effdet_conv_args* a, int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(a && (a->x || a->x_planes) && a->w && a->y, "conv2d: null tensor");
-    EFFDET_REQUIRE(!a->x_planes || (pw_gemm_eligible(a) && aligned16(a->x_planes)),
-                   "conv2d: x_planes is only understood by the tensor-core 1x1 path (Cin %% 8 == 0, no input prologue)");
-    EFFDET_REQUIRE(a->ksize == 1 || a->ksize == 3, "conv2d: ksize %d not in {1,3}", a->ksize);
-    EFFDET_REQUIRE(!a->tc_single || a->w_tc, "conv2d: tc_single needs the tensor-core weight pack w_tc (the exact-fp32 path has one product)");
-    EFFDET_REQUIRE(!a->tc_single || a->ksize == 3, "conv2d: tc_single is defined for 3x3 convolutions only (ksize %d)", a->ksize);
-    EFFDET_REQUIRE(a->Cin % 4 == 0 && a->Cout % 4 == 0, "conv2d: Cin=%d Cout=%d must be multiples of 4", a->Cin, a->Cout);
-    EFFDET_REQUIRE(a->B > 0 && a->H > 0 && a->W > 0, "conv2d: empty shape");
-    EFFDET_REQUIRE((a->scale == nullptr) == (a->shift == nullptr), "conv2d: scale/shift must come together");
-    EFFDET_REQUIRE((a->in_scale == nullptr) == (a->in_shift == nullptr) && (!a->in_scale || a->ksize == 1),
-                   "conv2d: in_scale/in_shift must come together (1x1 convs only: zero padding is applied after the activation)");
-    EFFDET_REQUIRE(aligned16(a->in_scale) && aligned16(a->in_shift), "conv2d: in_scale/in_shift must be 16-byte aligned");
-    EFFDET_REQUIRE(aligned16(a->x) && aligned16(a->w) && aligned16(a->y) && aligned16(a->z) && aligned16(a->bias) &&
-                       aligned16(a->residual) && aligned16(a->mask_src) && aligned16(a->a_scale),
-                   "conv2d: pointers must be 16-byte aligned");
-    EFFDET_REQUIRE(a->x_bstride % 4 == 0 && a->y_bstride % 4 == 0 && a->r_bstride % 4 == 0 && a->m_bstride % 4 == 0,
-                   "conv2d: batch strides must be multiples of 4 elements");
-    EFFDET_DEVICE(device);
-    const long long Mll = (long long)a->B * a->H * a->W;
-    EFFDET_REQUIRE(Mll < (1ll << 31), "conv2d: B*H*W too large");
-    const int M = (int)Mll, HW = a->H * a->W;
-    if (pw_gemm_eligible(a)) return pw_gemm_launch(a, (cudaStream_t)stream);
-    if (conv_tc_eligible(a)) return conv_tc_launch(a, 1, (cudaStream_t)stream);
+int conv_simt_launch(const effdet_conv_args* a, cudaStream_t st) {
+    const int M = a->B * a->H * a->W, HW = a->H * a->W;
     // pick the N tile that wastes the fewest padded columns (ties -> wider tile)
     int best = 128;
     long long best_pad = (long long)cdiv(a->Cout, 128) * 128;
@@ -403,7 +366,6 @@ extern "C" int effdet_conv2d(const effdet_conv_args* a, int device, effdet_strea
         long long padn = (long long)cdiv(a->Cout, bn) * bn;
         if (padn < best_pad) { best_pad = padn; best = bn; }
     }
-    cudaStream_t st = (cudaStream_t)stream;
     dim3 grid(cdiv(M, kBM), cdiv(a->Cout, best));
     if (best == 128) conv_igemm_kernel<128, 8><<<grid, kNT, 0, st>>>(*a, M, HW);
     else if (best == 64) conv_igemm_kernel<64, 4><<<grid, kNT, 0, st>>>(*a, M, HW);
@@ -411,53 +373,22 @@ extern "C" int effdet_conv2d(const effdet_conv_args* a, int device, effdet_strea
     return launch_status("conv_igemm_kernel");
 }
 
-static int colsum_launch(const float* x, float* out, long long M, int N, long long HW, long long bstride, int device,
-                         effdet_stream_t stream) {
+int colsum_launch(const float* x, float* out, long long M, int N, long long HW, long long bstride, cudaStream_t st) {
     EFFDET_REQUIRE(x && out && M > 0 && N > 0 && N % 4 == 0, "colsum: bad arguments");
     EFFDET_REQUIRE(aligned16(x), "colsum: x must be 16-byte aligned");
-    EFFDET_DEVICE(device);
     const int cvecs = N / 4;
     const int rows = rowpack_rows(cvecs);
     // ~4 waves of blocks, at least 8 row-iterations per block
     long long rpb = (M + num_sms() * 4 - 1) / (num_sms() * 4);
     if (rpb < (long long)rows * 8) rpb = (long long)rows * 8;
     dim3 grid(cdiv(M, rpb), rowpack_chunks(cvecs));
-    colsum_kernel<<<grid, kNT, 0, (cudaStream_t)stream>>>(x, out, M, N, (int)rpb, HW, bstride);
+    colsum_kernel<<<grid, kNT, 0, st>>>(x, out, M, N, (int)rpb, HW, bstride);
     return launch_status("colsum_kernel");
 }
 
-extern "C" int effdet_conv2d_wgrad(const effdet_wgrad_args* a, int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(a && (a->x || a->x_planes) && (a->dy || a->dy_planes) && a->dw, "wgrad: null tensor");
-    EFFDET_REQUIRE(!a->dy_planes || (a->precision == 1 && !a->dbias && aligned16(a->dy_planes) && (a->ws_x || a->x_planes)),
-                   "wgrad: dy_planes needs precision 1, no dbias and the ws_x workspace (or x_planes)");
-    EFFDET_REQUIRE(!a->x_planes || (a->precision == 1 && !a->a_scale && !a->in_scale && aligned16(a->x_planes) &&
-                                    (a->ws_dy || a->dy_planes)),
-                   "wgrad: x_planes needs precision 1 and no input prologue");
-    EFFDET_REQUIRE(a->ksize == 1 || a->ksize == 3, "wgrad: ksize %d not in {1,3}", a->ksize);
-    EFFDET_REQUIRE(!a->tc_single || a->precision == 1, "wgrad: tc_single needs precision 1 (the exact-fp32 path has one product)");
-    EFFDET_REQUIRE(!a->tc_single || a->ksize == 3, "wgrad: tc_single is defined for 3x3 convolutions only (ksize %d)", a->ksize);
-    EFFDET_REQUIRE(a->Cin % 4 == 0 && a->Cout % 4 == 0, "wgrad: channels must be multiples of 4");
-    EFFDET_REQUIRE(aligned16(a->x) && aligned16(a->dy) && aligned16(a->a_scale) && aligned16(a->in_scale) && aligned16(a->in_shift),
-                   "wgrad: pointers must be 16-byte aligned");
-    EFFDET_REQUIRE((a->in_scale == nullptr) == (a->in_shift == nullptr) && (!a->in_scale || a->ksize == 1),
-                   "wgrad: in_scale/in_shift must come together (1x1 convs only)");
-    EFFDET_REQUIRE(a->x_bstride % 4 == 0 && a->dy_bstride % 4 == 0, "wgrad: batch strides must be multiples of 4");
-    EFFDET_DEVICE(device);
-    const long long Mll = (long long)a->B * a->H * a->W;
-    EFFDET_REQUIRE(Mll < (1ll << 31), "wgrad: B*H*W too large");
-    const int M = (int)Mll, HW = a->H * a->W;
+int wgrad_simt_launch(const effdet_wgrad_args* a, cudaStream_t st) {
+    const int M = a->B * a->H * a->W, HW = a->H * a->W;
     const int taps = a->ksize * a->ksize;
-    cudaStream_t st = (cudaStream_t)stream;
-    int s = EFFDET_OK;
-    bool dbias_done = false;
-    if (pw_wgrad_eligible(a)) {
-        s = pw_wgrad_launch(a, st);      // 1x1, no bias: operands converted in the kernel, no split passes
-    } else if (wgrad_tc_eligible(a)) {
-        s = wgrad_tc_launch(a, st, &dbias_done);
-    } else if (a->dy_planes || a->x_planes) {
-        return fail(EFFDET_ERR_UNSUPPORTED, "wgrad: dy_planes given but the TMA-fed tensor-core kernel cannot take this shape or "
-                                            "input prologue (check effdet_wgrad_tc_geometry_ok first)");
-    } else {
     int BC, BN;
     if (a->Cin <= 32) { BC = 32; BN = 128; }
     else if (a->Cout <= 48) { BC = 128; BN = 32; }
@@ -476,12 +407,12 @@ extern "C" int effdet_conv2d_wgrad(const effdet_wgrad_args* a, int device, effde
     else if (BN == 32) conv_wgrad_kernel<128, 32, 4, 4><<<grid, kNT, 0, st>>>(*a, M, HW, cps, ctiles);
     else if (BC == 128) conv_wgrad_kernel<128, 128, 8, 8><<<grid, kNT, 0, st>>>(*a, M, HW, cps, ctiles);
     else conv_wgrad_kernel<64, 64, 4, 4><<<grid, kNT, 0, st>>>(*a, M, HW, cps, ctiles);
-    s = launch_status("conv_wgrad_kernel");
-    }
-    if (s) return s;
-    if (a->dbias && !dbias_done) return colsum_launch(a->dy, a->dbias, M, a->Cout, HW, a->dy_bstride, device, stream);
-    return EFFDET_OK;
+    return launch_status("conv_wgrad_kernel");
 }
+
+}  // namespace effdet
+
+using namespace effdet;
 
 extern "C" int effdet_pack_conv_weight(const float* w_oihw, float* w_fwd, float* w_dgrad, int Cout, int Cin, int ksize,
                                        int device, effdet_stream_t stream) {

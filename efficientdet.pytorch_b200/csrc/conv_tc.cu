@@ -48,7 +48,6 @@ struct FwdSmem {
 // Several pyramid levels that share one weight tensor (RetinaHead runs the same convs on P3..P7,
 // models/retinahead.py:131-132) in ONE launch: the M tiles of all levels are concatenated so the small
 // levels (a handful of CTAs each) ride along with the large ones instead of paying their own latency-bound launch.
-constexpr int kMaxLevels = 8;
 struct ConvMultiArgs {
     ConvLevel lv[kMaxLevels];
     int tile_begin[kMaxLevels + 1];
@@ -353,7 +352,6 @@ wgrad_tc_kernel(const __grid_constant__ WgradPrefix pa, const int M, const int H
 // one long GEMM-K dimension, so one launch covers them all; each chunk looks up its level's tensor
 // maps and pixel-box geometry.
 // ---------------------------------------------------------------------------------------------
-constexpr int kWgMaxLevels = 8;
 struct WgMaps {
     CUtensorMap dy[kWgMaxLevels];
     CUtensorMap x[kWgMaxLevels];
@@ -500,12 +498,6 @@ EncodeTiledFn encode_fn() {
 
 int conv_tc_kpad(int k) { return (k + kTileK - 1) / kTileK * kTileK; }
 
-bool conv_tc_eligible(const effdet_conv_args* a) {
-    // the 3x3 convs of neck and head; the MBConv prologue / epilogue inputs are served by the CUDA-core kernel
-    return a->w_tc != nullptr && a->ksize == 3 && a->Cin % 4 == 0 && a->Cout % 4 == 0 && a->Cout >= 16 && !a->a_scale &&
-           !a->z && !a->scale && !a->shift && !a->row_scale && !a->in_scale;
-}
-
 // 3-D tensor map over K-major bf16 hi/lo planes [2][rows][k]: boxes of 64 k (one 128-byte swizzled row) x box_rows rows
 int kmajor_planes_map(EncodeTiledFn enc, CUtensorMap* map, const void* base, int rows, int k, int box_rows) {
     const cuuint64_t gdim[3] = {(cuuint64_t)k, (cuuint64_t)rows, 2};
@@ -552,14 +544,6 @@ int conv_tc_launch(const effdet_conv_args* levels, int nlevels, cudaStream_t st)
     return launch_smem("conv_tc_kernel", conv_tc_kernel<128, 3, 3>, grid, kTcThreads, FwdSmem<128, 3>::kBytes, st, map, ma, kblocks);
 }
 
-bool wgrad_tc_eligible(const effdet_wgrad_args* a) {
-    // the tensor-core weight gradients have no input prologue: those convs go to the CUDA-core kernel
-    if (a->precision != 1 || a->Cin % 4 || a->Cout % 4 || a->Cin < 16 || a->Cout < 16 || a->a_scale || a->in_scale) return false;
-    WgGeom g;
-    const bool tma_ok = (a->ws_x || a->x_planes) && (a->ws_dy || a->dy_planes) && wg_geometry(a->B, a->H, a->W, &g);
-    return tma_ok || (!a->dy_planes && !a->x_planes);     // the gathering kernel reads fp32 operands only
-}
-
 bool wg_geometry(int B, int H, int W, WgGeom* g) {
     const int Wb = W <= 64 ? W : 64;
     if (W % Wb) return false;
@@ -591,11 +575,10 @@ int planes_map(EncodeTiledFn enc, CUtensorMap* map, void* base, int B, int H, in
     return EFFDET_OK;
 }
 
-// TMA-fed weight gradient of one shared-weight layer over all levels in one launch; returns 1 when some level cannot use
-// it (no legal pixel box, no plane workspace, an input prologue) and the caller falls back
-static int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t st) {
+// TMA-fed weight gradient of one shared-weight layer over all levels in one launch.  conv_api.cu has checked that every
+// level has a pixel box and both operands as planes or plane workspaces, and that the tensor-map encoder is available.
+int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t st) {
     EncodeTiledFn enc = encode_fn();
-    if (!enc || nlevels > kWgMaxLevels) return 1;
     WgMaps maps;
     WgMultiArgs ma;
     memset(&ma, 0, sizeof(ma));
@@ -604,9 +587,7 @@ static int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaSt
     int chunks = 0;
     for (int l = 0; l < nlevels; ++l) {
         const effdet_wgrad_args* a = &levels[l];
-        if (!(a->ws_x || a->x_planes) || !(a->ws_dy || a->dy_planes) || a->a_scale || a->in_scale ||
-            !wg_geometry(a->B, a->H, a->W, &ma.g[l]))
-            return 1;
+        wg_geometry(a->B, a->H, a->W, &ma.g[l]);
         ma.chunk_begin[l] = chunks;
         chunks += ma.g[l].nbx * ma.g[l].nby * ma.g[l].nbb;
     }
@@ -659,12 +640,9 @@ static int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaSt
                        ma, cps, ctiles);
 }
 
-int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st, bool* dbias_done) {
-    const int r = wgrad_tc2_launch(a, 1, st);
-    *dbias_done = r == 0;       // the TMA path folds the bias gradient into its dy split pass
-    if (r <= 0) return r;       // launched (0) or failed (<0); 1 = geometry unsupported -> gather kernel
-    const long long Mll = (long long)a->B * a->H * a->W;
-    const int M = (int)Mll, HW = a->H * a->W;
+// weight gradient of one level from fp32 operands that the kernel gathers itself; the bias gradient is not part of it
+int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st) {
+    const int M = a->B * a->H * a->W, HW = a->H * a->W;
     const int taps = a->ksize * a->ksize;
     const int BC = a->Cin > 64 ? 256 : 64;
     const int ctiles = cdiv(a->Cin, BC), ntiles = cdiv(a->Cout, kTileM);
@@ -698,60 +676,6 @@ extern "C" int effdet_conv_tc_kpad(int channels) { return conv_tc_kpad(channels)
 extern "C" int effdet_wgrad_tc_geometry_ok(int B, int H, int W) {
     WgGeom g;
     return wg_geometry(B, H, W, &g) ? 1 : 0;
-}
-
-extern "C" int effdet_conv2d_wgrad_multi(const effdet_wgrad_args* levels, int nlevels, int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(levels && nlevels >= 1, "conv2d_wgrad_multi: no levels");
-    bool same = true;
-    for (int l = 0; l < nlevels; ++l) {
-        const effdet_wgrad_args* a = &levels[l];
-        EFFDET_REQUIRE((a->x || a->x_planes) && (a->dy || a->dy_planes) && a->dw, "conv2d_wgrad_multi: null tensor");
-        EFFDET_REQUIRE(!(a->dy_planes && a->dbias), "conv2d_wgrad_multi: dy_planes excludes dbias (the producer supplies the column sums)");
-        EFFDET_REQUIRE(a->tc_single == levels[0].tc_single, "conv2d_wgrad_multi: levels disagree on tc_single");
-        EFFDET_REQUIRE(!a->tc_single || (a->precision == 1 && a->ksize == 3),
-                       "conv2d_wgrad_multi: tc_single needs precision 1 and a 3x3 convolution");
-        same = same && a->dw == levels[0].dw && a->dbias == levels[0].dbias && a->Cin == levels[0].Cin &&
-               a->Cout == levels[0].Cout && a->ksize == levels[0].ksize && a->precision == 1 && wgrad_tc_eligible(a);
-    }
-    if (same && nlevels > 1) {          // one level: effdet_conv2d_wgrad checks its arguments and takes the same kernel
-        EFFDET_DEVICE(device);
-        const int r = wgrad_tc2_launch(levels, nlevels, (cudaStream_t)stream);
-        if (r < 0) return r;
-        if (r == 0) return EFFDET_OK;          // bias gradient was fused into the dy split pass
-    }
-    for (int l = 0; l < nlevels; ++l) {
-        const int s = effdet_conv2d_wgrad(&levels[l], device, stream);
-        if (s) return s;
-    }
-    return EFFDET_OK;
-}
-
-extern "C" int effdet_conv2d_multi(const effdet_conv_args* levels, int nlevels, int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(levels && nlevels >= 1 && nlevels <= kMaxLevels, "conv2d_multi: 1..%d levels", kMaxLevels);
-    bool tc = true;
-    for (int l = 0; l < nlevels; ++l) {
-        const effdet_conv_args* a = &levels[l];
-        EFFDET_REQUIRE(a->x && a->w && a->y, "conv2d_multi: null tensor");
-        EFFDET_REQUIRE(a->Cin == levels[0].Cin && a->Cout == levels[0].Cout && a->ksize == levels[0].ksize &&
-                           a->act == levels[0].act && a->w == levels[0].w && a->w_tc == levels[0].w_tc &&
-                           a->bias == levels[0].bias,
-                       "conv2d_multi: all levels must share weights, bias, channels and activation");
-        EFFDET_REQUIRE(a->tc_single == levels[0].tc_single, "conv2d_multi: levels disagree on tc_single");
-        EFFDET_REQUIRE(!a->tc_single || (a->w_tc && a->ksize == 3), "conv2d_multi: tc_single needs w_tc and a 3x3 convolution");
-        tc = tc && conv_tc_eligible(a) && (long long)a->B * a->H * a->W < (1ll << 31);
-        EFFDET_REQUIRE(aligned16(a->x) && aligned16(a->y) && aligned16(a->residual) && aligned16(a->mask_src) &&
-                           a->x_bstride % 4 == 0 && a->y_bstride % 4 == 0 && a->r_bstride % 4 == 0 && a->m_bstride % 4 == 0,
-                       "conv2d_multi: alignment");
-    }
-    if (tc && nlevels > 1) {          // one level: effdet_conv2d checks its arguments and takes the same kernel
-        EFFDET_DEVICE(device);
-        return conv_tc_launch(levels, nlevels, (cudaStream_t)stream);
-    }
-    for (int l = 0; l < nlevels; ++l) {          // exact-fp32 mode / unsupported shapes: one launch per level
-        int s = effdet_conv2d(&levels[l], device, stream);
-        if (s) return s;
-    }
-    return EFFDET_OK;
 }
 
 extern "C" int effdet_pack_conv_weight_tc(const float* w_oihw, void* w_fwd, void* w_dgrad, int Cout, int Cin, int ksize,

@@ -290,15 +290,6 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     }
 }
 
-bool pw_gemm_eligible(const effdet_conv_args* a) {
-    if (a->ksize != 1 || a->w_tc == nullptr || a->Cin % 4 || a->Cout % 4 || a->Cin < 8 || a->Cout < 8) return false;
-    const long long HW = (long long)a->H * a->W;
-    if (a->x_planes) return a->Cin % 8 == 0 && !a->in_scale && !a->a_scale && (long long)a->B * HW < (1ll << 31);
-    if (a->x_bstride != HW * a->Cin) return false;              // x must be one dense [M, Cin] matrix for the 2-D tensor map
-    if ((long long)a->B * HW >= (1ll << 31)) return false;
-    return true;
-}
-
 int pw_gemm_launch(const effdet_conv_args* a, cudaStream_t st) {
     EncodeTiledFn enc = encode_fn();
     if (!enc) return fail(EFFDET_ERR_UNSUPPORTED, "conv2d(pw): cuTensorMapEncodeTiled unavailable");

@@ -224,15 +224,6 @@ __global__ void __launch_bounds__(kWgThreads, 1) pw_wgrad_kernel(const __grid_co
     }
 }
 
-bool pw_wgrad_eligible(const effdet_wgrad_args* a) {
-    if (a->ksize != 1 || a->precision != 1 || a->dbias || a->x_planes || !a->x) return false;
-    if (a->Cin % 8 || a->Cout % 8 || a->Cin < 8 || a->Cout < 8) return false;
-    const long long HW = (long long)a->H * a->W;
-    if (a->x_bstride != HW * a->Cin) return false;
-    if (!a->dy_planes && (!a->dy || a->dy_bstride != HW * a->Cout)) return false;
-    return (long long)a->B * HW < (1ll << 31) - 64;
-}
-
 int pw_wgrad_launch(const effdet_wgrad_args* a, cudaStream_t st) {
     PwWgParams P;
     memset(&P, 0, sizeof(P));

@@ -306,6 +306,10 @@ struct alignas(8) ArgsPrefix {
 using ConvLevel = ArgsPrefix<effdet_conv_args, offsetof(effdet_conv_args, tc_single)>;
 using WgradPrefix = ArgsPrefix<effdet_wgrad_args, offsetof(effdet_wgrad_args, tc_single)>;
 
+// pyramid levels one launch of conv_tc_kernel / wgrad_tc2_multi_kernel covers (conv_tc.cu)
+constexpr int kMaxLevels = 8;
+constexpr int kWgMaxLevels = 8;
+
 // Pixel boxes of the TMA-fed kernels: a [B,H,W,*] map is tiled into boxes of Wb x Hb x Bb = kstage pixels (16..64, a
 // multiple of 16) that one tensor-map load turns into kstage consecutive 128-byte rows of shared memory (conv_tc.cu)
 struct WgGeom {

@@ -294,9 +294,15 @@ def conv_wgrad_raw(dev_t, x_ptr, x_bs, dy_ptr, dy_bs, dw, dbias, B, H, W, Cin, C
     N.call('effdet_conv2d_wgrad', dev_t, a)
 
 
+def pixel_boxes_ok(maps):
+    """do the TMA-fed tensor-core kernels find a pixel box for every map?  maps: (B, H, W, ...) shapes"""
+    lib = N.load()
+    return all(lib.effdet_wgrad_tc_geometry_ok(m[0], m[1], m[2]) for m in maps)
+
+
 def planes_ok(B, H, W, C):
     """can a [B,H,W,C] gradient be handed to the tensor-core weight / data gradients as bf16 hi/lo planes?"""
-    return tc_enabled() and C % 8 == 0 and bool(N.load().effdet_wgrad_tc_geometry_ok(B, H, W))
+    return tc_enabled() and C % 8 == 0 and pixel_boxes_ok([(B, H, W)])
 
 
 def conv_wgrad_multi(dev_t, levels, dw, dbias, Cin, Cout, k, tc=False):
@@ -609,8 +615,7 @@ class BiFPNLayerFn(torch.autograd.Function):
 
         # tensor-core mode: the fused map is written as bf16 hi/lo planes and the node conv is the TMA-fed planes
         # kernel (no gather, no split pass in the weight gradient); every level must admit a TMA pixel box
-        pl = tc_enabled() and C % 4 == 0 and all(N.load().effdet_wgrad_tc_geometry_ok(t.shape[0], t.shape[1], t.shape[2])
-                                                 for t in ins)
+        pl = tc_enabled() and C % 4 == 0 and pixel_boxes_ok(t.shape for t in ins)
 
         def conv(idx, f, like):
             if pl:
@@ -851,13 +856,8 @@ def wgrad_planes_multi(dev_t, levels, dw, Cin, Cout, k):
 
 def head_planes_ok(feats, params):
     """can the RetinaHead run with activations kept as bf16 hi/lo planes (TMA-fed tensor-core path)?"""
-    if not tc_enabled():
+    if not tc_enabled() or any(f.shape[3] % 4 for f in feats) or not pixel_boxes_ok(f.shape for f in feats):
         return False
-    lib = N.load()
-    for f in feats:
-        B, H, W, C = f.shape
-        if C % 4 or not lib.effdet_wgrad_tc_geometry_ok(B, H, W):
-            return False
     return all(p.shape[0] % 4 == 0 and p.shape[0] >= 16 for p in params[0::2])
 
 

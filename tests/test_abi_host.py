@@ -95,6 +95,49 @@ def test_argument_refusals_and_error_plumbing(native):
         assert lib.effdet_add(fake, fake, fake, 64, 0, None) < 0 and 'cuda' in err().lower()
 
 
+def test_multi_level_convolutions_check_every_level(native):
+    """the multi-level dense-convolution entry points refuse, with the single-level message, whatever the single-level
+    call refuses on any level -- also when the levels would otherwise share one tensor-core launch -- and they refuse
+    before any device work, so these calls run without a GPU"""
+    import ctypes
+    lib = native.load()
+
+    def err():
+        return lib.effdet_last_error().decode()
+
+    fake = 1 << 20                                           # aligned non-null "pointer"; never dereferenced
+
+    def wg(**kw):                                            # a level the TMA-fed weight-gradient kernel would take
+        a = native.WgradArgs(x=fake, x_bstride=8 * 8 * 64, dy=fake, dy_bstride=8 * 8 * 64, dw=fake, B=2, H=8, W=8,
+                             Cin=64, Cout=64, ksize=3, precision=1, ws_x=fake, ws_dy=fake)
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+
+    def wgrad_multi(*levels):
+        return lib.effdet_conv2d_wgrad_multi((native.WgradArgs * len(levels))(*levels), len(levels), 0, None)
+
+    assert wgrad_multi(wg(), wg(x=fake + 4)) == -1 and err() == 'wgrad: pointers must be 16-byte aligned'
+    assert wgrad_multi(wg(), wg(x_bstride=8 * 8 * 64 + 2)) == -1 and err().startswith('wgrad: batch strides')
+    assert wgrad_multi(wg(ksize=5), wg(ksize=5)) == -1 and err() == 'wgrad: ksize 5 not in {1,3}'
+    assert wgrad_multi(wg(), wg(B=0)) == -1 and err() == 'wgrad: empty shape'
+    assert lib.effdet_conv2d_wgrad(ctypes.byref(wg(W=0)), 0, None) == -1 and err() == 'wgrad: empty shape'
+    assert wgrad_multi(wg(), wg(dw=fake + 4096)) == -1 and 'share dw' in err()
+    assert lib.effdet_conv2d_wgrad(None, 0, None) == -1 and err() == 'wgrad: null tensor'
+
+    def conv(**kw):                                          # a level the tensor-core implicit GEMM would take
+        a = native.ConvArgs(x=fake, x_bstride=8 * 8 * 64, w=fake, y=fake, y_bstride=8 * 8 * 64, B=2, H=8, W=8, Cin=64,
+                            Cout=64, ksize=3, w_tc=fake)
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+
+    arr = (native.ConvArgs * 2)(conv(), conv(B=0))
+    assert lib.effdet_conv2d_multi(arr, 2, 0, None) == -1 and err() == 'conv2d: empty shape'
+    arr = (native.ConvArgs * 2)(conv(), conv(y=fake + 4))
+    assert lib.effdet_conv2d_multi(arr, 2, 0, None) == -1 and err() == 'conv2d: pointers must be 16-byte aligned'
+
+
 @pytest.mark.parametrize('net,W,D', [('efficientdet-d0', 64, 2), ('efficientdet-d3', 160, 5)])
 def test_state_dict_schema_matches_reference(net, W, D):
     from models import EfficientDet
