@@ -32,6 +32,10 @@ constexpr int kTcThreads = 288;        // two gather / MMA / epilogue warpgroups
 constexpr int kTcProducers = 256;      // the two warpgroups (all of the gathering weight-gradient kernel)
 constexpr int kTileM = 128;     // pixels per CTA (fwd/dgrad) or output channels per CTA (wgrad)
 constexpr int kTileK = 64;      // bf16 elements per 128-byte swizzled row
+// Most pixel chunks (<= 64 pixels each) one weight-gradient CTA accumulates in its wgmma fp32 accumulator.  That
+// accumulation's error grows linearly with the K steps it covers (H100, bf16x3, whole-tensor norm-relative: 4.5e-6 at
+// <= 12 chunks, 1.0e-5 at 43, 1.9e-5 at 86, 3.8e-5 at 171), so long K ranges are split further and added by atomics.
+constexpr int kWgMaxChunksPerSplit = 64;
 
 // ---------------------------------------------------------------------------------------------
 // forward / data-gradient kernel
@@ -619,10 +623,12 @@ int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t 
     const int taps = a0->ksize * a0->ksize;
     const int BC = a0->Cin > 64 ? 256 : 64;
     const int ctiles = cdiv(a0->Cin, BC), ntiles = cdiv(a0->Cout, kTileM);
-    // split-K so that the grid is as close as possible to (but not above) two full waves of CTAs
+    // split-K so that the grid is as close as possible to (but not above) two full waves of CTAs, and no CTA accumulates
+    // more than kWgMaxChunksPerSplit chunks.  tests/test_planes_path_parity.py (_split_plan) mirrors this arithmetic.
     int splits = (num_sms() * 2) / (ctiles * ntiles * taps);
     if (splits < 1) splits = 1;
     if (splits > cdiv(chunks, 4)) splits = cdiv(chunks, 4);
+    if (splits < cdiv(chunks, kWgMaxChunksPerSplit)) splits = cdiv(chunks, kWgMaxChunksPerSplit);
     int cps = cdiv(chunks, splits);
     splits = cdiv(chunks, cps);
     dim3 grid(ctiles * ntiles, taps, splits);
@@ -650,6 +656,7 @@ int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st) {
     int splits = cdiv(num_sms() * 2, ctiles * ntiles * taps);
     if (splits < 1) splits = 1;
     if (splits > cdiv(nchunks, 8)) splits = cdiv(nchunks, 8);
+    if (splits < cdiv(nchunks, kWgMaxChunksPerSplit)) splits = cdiv(nchunks, kWgMaxChunksPerSplit);
     int cps = cdiv(nchunks, splits);
     splits = cdiv(nchunks, cps);
     dim3 grid(ctiles * ntiles, taps, splits);
