@@ -159,6 +159,8 @@ SIGNATURES = {
     'effdet_gather_detections_batch': [_P, _P, _P, _P, _P, _INT, _INT, _INT, _P, _P, _P] + _TAIL,
     'effdet_multi_sumsq': [_P, _P, _P, _P, _INT, _INT, _P] + _TAIL,
     'effdet_multi_clip_adamw': [_P] * 7 + [_INT, _INT, _P] + [_F] * 8 + [_INT] + _TAIL,
+    'effdet_multi_accumulate': [_P] * 5 + [_INT, _INT] + [_P] * 3 + _TAIL,
+    'effdet_multi_clip_adamw_dev': [_P] * 7 + [_INT, _INT, _P, _F] + [_P] * 4 + [ctypes.c_double] * 2 + [_F] * 2 + _TAIL,
     'effdet_normalize_pad': [_P, _P, _P, _P, _P, _INT, _INT, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)] + _TAIL,
     'effdet_collate_annots': [_P, _P, _P, _P, _P, _P, _INT, _INT] + _TAIL,
     'effdet_eval_select': [_P, _P, _P, _INT, _F, _F, _INT, _INT, _P, _P, _P, _P] + _TAIL,

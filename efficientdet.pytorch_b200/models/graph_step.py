@@ -10,19 +10,53 @@ one cudaGraphLaunch, which matters as soon as the GPU finishes a step faster tha
     loss = step(images, annotations)      # copies into the static inputs, replays, returns the static loss tensor
     ... model parameters' .grad now hold this step's gradients (same tensors every step)
 
+Without an optimizer the graph reads the packed weights / folded BatchNorm its warm-up derived into the caches of
+models/_ops.py; anything that invalidates them (load_state_dict, train(), eval(), freeze_bn(), building a step with an
+optimizer) means building this step again.
+
 Build it BEFORE any eager step, or after every reference to earlier eager losses / outputs has been dropped: a live autograd
 graph keeps the parameters' gradient accumulators bound to the stream it ran on (the legacy stream), and the engine
 may not touch that stream while another one is capturing.
 
 Shapes are static (the reference pads every batch to the common size and a fixed annotation count per batch can be
 obtained by padding with -1 rows, which FocalLoss ignores).  Drop-connect keeps working: torch.rand inside a captured
-region advances the Philox offset on every replay.  With `optimizer=FusedClipAdamW(...)` the clip + AdamW launches are
-captured too; the packed-weight / folded-BN derivations are then captured as well (they must re-run every step because
-the weights change without Python seeing it).
+region advances the Philox offset on every replay.
+
+Training with the optimizer in the graph.  With `optimizer=FusedClipAdamW(...)` every call is one micro-step of the
+reference loop (train.py:95-133): forward, loss, backward, gradients added to the persistent accumulators that
+`p.grad` then refers to (skipped when the loss is exactly 0), and, when `update` is true and the loss is non-zero, the
+clip + AdamW update, which also empties the accumulators.  The loop as a user writes it, with k =
+--grad_accumulation_steps:
+
+    opt = FusedClipAdamW(model.parameters(), lr=lr, max_norm=0.1)    # opt.load_state_dict(...) here, if resuming
+    scheduler = torch.optim.lr_scheduler.ReduceLROnPlateau(opt, patience=3)
+    step = GraphedTrainStep(model, images_example, annotations_example, optimizer=opt)
+    for epoch in range(num_epoch):
+        opt.zero_grad()
+        losses = []
+        for idx, (images, annotations) in enumerate(train_loader):
+            loss = step(images, annotations, update=(idx + 1) % k == 0)
+            losses.append(loss.clone())                    # stays on the device: no synchronisation per step
+        losses = torch.stack(losses)
+        scheduler.step(float(losses[losses != 0].mean()))  # the reference averages the non-skipped losses
+        torch.save({'optimizer': opt.state_dict(), ...})  # true step counts: one device read
+
+The step counters and learning rates live in device memory: each call writes the `update` flag, and the lr of any
+param group whose `group['lr']` changed, into their device scalars before the replay (launches, no synchronisation),
+so schedulers work without recapture.  betas, eps, weight_decay and max_norm are fixed at capture; changing them
+raises.  Building the step leaves parameters, moments and step counts untouched: the warm-up runs forward and backward
+only.  Under DDP every call must update (`update=True`); gradient accumulation across DDP micro-steps is not
+supported.  Any other optimizer has its `step()` captured as is (the warm-up then runs it too) and allows
+`update=True` only.
+
+With an optimizer in the graph the packed-weight / folded-BN derivations are captured as well: they re-run on every
+replay because the weights change without Python seeing it.  For the same reason, eager use of the model between
+replays needs `model.eval()` / `model.train()` (or `_ops.invalidate_caches()`) first.
 """
 import torch
 
 from . import _ops
+from .fused_optim import FusedClipAdamW
 
 
 class GraphedTrainStep:
@@ -39,6 +73,7 @@ class GraphedTrainStep:
             warmup = max(warmup, 11)
         self.model = model
         self.optimizer = optimizer
+        self.fused = isinstance(optimizer, FusedClipAdamW)
         self.static_images = images.clone()
         self.static_annots = annotations.clone()
         params = [p for p in model.parameters() if p.requires_grad]
@@ -51,13 +86,15 @@ class GraphedTrainStep:
         torch.cuda.synchronize(images.device)
         if optimizer is not None:
             _ops.invalidate_caches()                                  # capture the weight re-packing with the step
+        if self.fused:
+            optimizer._bind_graph([p for p in params if p.grad is not None])
         self.graph = torch.cuda.CUDAGraph()
         for p in params:
             p.grad = None
         n0 = _ops.N.launch_count()
         try:
             with torch.cuda.graph(self.graph):
-                self.static_loss = self._eager_step(params, zero=False)
+                self.static_loss = self._eager_step(params, zero=False, capture=True)
         except RuntimeError as e:
             if 'legacy stream' in str(e) or 'previous error during capture' in str(e):
                 raise _ops.N.EffdetNativeError(
@@ -68,8 +105,12 @@ class GraphedTrainStep:
             raise
         self.library_launches = _ops.N.launch_count() - n0            # kernels of this library recorded into the graph
         self.params = params
+        if self.fused:
+            optimizer._graph_captured()
+            # capture recorded the weight packing without running it: eager calls derive their own until a replay
+            _ops.invalidate_caches()
 
-    def _eager_step(self, params, zero=True):
+    def _eager_step(self, params, zero=True, capture=False):
         if zero:
             for p in params:
                 p.grad = None
@@ -84,11 +125,24 @@ class GraphedTrainStep:
             grads = torch.autograd.grad(loss, params, allow_unused=True)
             for p, g in zip(params, grads):
                 p.grad = g
-        if self.optimizer is not None:
+        if self.fused:
+            if capture:                                              # the warm-up leaves the optimizer untouched
+                self.optimizer._graph_launch({p: p.grad for p in params}, loss)
+        elif self.optimizer is not None:
             self.optimizer.step()
         return loss.detach()
 
-    def __call__(self, images, annotations):
+    def __call__(self, images, annotations, update=True):
+        """One micro-step.  update: run the optimizer after it (train.py:115 `(idx + 1) % k == 0`); with
+        FusedClipAdamW the update is skipped on the device when the step's loss is exactly zero."""
+        if self.fused:
+            if self.ddp and not update:
+                raise _ops.N.EffdetNativeError('GraphedTrainStep: update=False (gradient accumulation) is not supported '
+                                               'under DistributedDataParallel; call it with update=True')
+            self.optimizer._graph_prepare(update)
+        elif not update:
+            raise _ops.N.EffdetNativeError('GraphedTrainStep: update=False (gradient accumulation) needs '
+                                           'optimizer=FusedClipAdamW(...)')
         self.static_images.copy_(images, non_blocking=True)
         self.static_annots.copy_(annotations, non_blocking=True)
         self.graph.replay()

@@ -364,6 +364,27 @@ int effdet_multi_clip_adamw(const uint64_t* p_ptrs, const uint64_t* g_ptrs, cons
                             const int64_t* chunk_off, int nchunks, int chunk, const float* norm_sq, float max_norm,
                             float lr, float beta1, float beta2, float eps, float weight_decay, float bias_c1,
                             float bias_c2, int write_clipped_grad, int device, effdet_stream_t stream);
+/* The same step replayed from a CUDA graph, with gradient accumulation (train.py:107-118 with
+ * --grad_accumulation_steps k): every value that changes between steps is read from device memory.
+ *   effdet_multi_accumulate     : acc_t[i] += g_t[i] for every tensor, unless loss[0] == 0.0f exactly (the reference's
+ *                                 `if bool(loss == 0): continue`), in which case nothing is written.  With gate given
+ *                                 (update_requested then too): gate[0] = update_requested[0] != 0 && loss[0] != 0.
+ *   effdet_multi_clip_adamw_dev : gate[0] == 0: returns without touching p, m, v, acc or the counter.  Otherwise the
+ *                                 update of effdet_multi_clip_adamw on g_ptrs = the accumulators, with lr = lr[0],
+ *                                 bias_c = (float)(1 - beta^(step[0] + 1)) in fp64 and 1 - beta rounded from fp64
+ *                                 (torch.optim.AdamW's rounding), then acc = 0 and step[0] += 1.
+ *                                 ticket: one zero-initialised uint32 that the launch returns to zero (it orders the
+ *                                 counter's advance after every CTA's read); launches sharing it must be stream-ordered.
+ * norm_sq for the update comes from effdet_multi_sumsq over the accumulators, zeroed before it. */
+int effdet_multi_accumulate(const uint64_t* acc_ptrs, const uint64_t* g_ptrs, const int64_t* numels,
+                            const int32_t* chunk_tensor, const int64_t* chunk_off, int nchunks, int chunk,
+                            const float* loss, const int32_t* update_requested, int32_t* gate, int device,
+                            effdet_stream_t stream);
+int effdet_multi_clip_adamw_dev(const uint64_t* p_ptrs, const uint64_t* g_ptrs, const uint64_t* m_ptrs,
+                                const uint64_t* v_ptrs, const int64_t* numels, const int32_t* chunk_tensor,
+                                const int64_t* chunk_off, int nchunks, int chunk, const float* norm_sq, float max_norm,
+                                const float* lr, int64_t* step, const int32_t* gate, uint32_t* ticket, double beta1,
+                                double beta2, float eps, float weight_decay, int device, effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) rank 2: the step BEFORE the hot path, on the device.  Normalizer + Augmenter (horizontal flip) + zero pad
