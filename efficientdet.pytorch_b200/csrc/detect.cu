@@ -7,7 +7,7 @@
 // Bit-exactness rules (the keep-set must equal torchvision's): fp32 IoU from separately rounded
 // ops (no FMA contraction), suppress iff IoU > thr compared in double, candidates ordered by
 // score descending with ties broken by lower anchor index (== stable sort of the masked list).
-#include "common.cuh"
+#include "bitonic.cuh"
 
 namespace effdet {
 
@@ -292,18 +292,22 @@ static int candidates_launch(const float* cls, const float* reg, const float* an
     int s = launch_status("detect_candidates_kernel");
     if (s) return s;
     // sort every image's segment ascending: best candidates first, sentinels last
-    const int n = B * npad;
-    const int chunk = npad < kChunk ? npad : kChunk;
+    return bitonic_sort_launch(keys, B * npad, npad, st);
+}
+
+int bitonic_sort_launch(uint64_t* keys, int n, int seg, cudaStream_t st) {
+    int s;
+    const int chunk = seg < kChunk ? seg : kChunk;
     if (chunk >= 2) {
-        bitonic_chunk_sort_kernel<<<n / chunk, 1024, chunk * sizeof(uint64_t), st>>>(keys, chunk, npad);
+        bitonic_chunk_sort_kernel<<<n / chunk, 1024, chunk * sizeof(uint64_t), st>>>(keys, chunk, seg);
         if ((s = launch_status("bitonic_chunk_sort_kernel"))) return s;
     }
-    for (int k = chunk * 2; k <= npad; k <<= 1) {
+    for (int k = chunk * 2; k <= seg; k <<= 1) {
         for (int j = k >> 1; j >= chunk; j >>= 1) {
-            bitonic_global_step_kernel<<<cdiv(n / 2, 256), 256, 0, st>>>(keys, n, npad, k, j);
+            bitonic_global_step_kernel<<<cdiv(n / 2, 256), 256, 0, st>>>(keys, n, seg, k, j);
             if ((s = launch_status("bitonic_global_step_kernel"))) return s;
         }
-        bitonic_chunk_merge_kernel<<<n / chunk, 1024, chunk * sizeof(uint64_t), st>>>(keys, chunk, npad, k);
+        bitonic_chunk_merge_kernel<<<n / chunk, 1024, chunk * sizeof(uint64_t), st>>>(keys, chunk, seg, k);
         if ((s = launch_status("bitonic_chunk_merge_kernel"))) return s;
     }
     return EFFDET_OK;

@@ -1,11 +1,11 @@
-// The steps either side of the hot path, on the device (SURVEY.md 8(f) ranks 2 and 3):
+// The step before the hot path, on the device (SURVEY.md 8(f) rank 2):
 //   input side  : Normalizer + Augmenter (horizontal flip) + zero-pad to the common size + collater + `.cuda().float()`
 //                 datasets/augmentation.py:69-91,111-150, train.py:105-106  (cv2.resize is NOT reproduced: images enter at
 //                 their final resolution; everything after the decode is otherwise done here)
-//   output side : score threshold + top-`max_detections` by score + per-class split of eval.py:108-128
+// (the output side, eval.py's selection, is in voc_eval.cu)
 // Arithmetic follows the reference's dtypes exactly so the results are bit-identical to NumPy:
 //   Normalizer computes (img.astype(float32) - mean[float64]) / std[float64] in float64 and train.py casts to float32 on
-//   the device; collater writes float64 annotations into a float32 tensor; eval.py divides float32 boxes by float32(scale).
+//   the device; collater writes float64 annotations into a float32 tensor.
 #include "common.cuh"
 
 namespace effdet {
@@ -66,67 +66,6 @@ __global__ void collate_annots_kernel(const double* __restrict__ rows, const int
     o[4] = (float)r[4];
 }
 
-// eval.py:108-128 for one image.  One CTA.  Input rows are the model's detections (any order); a row is selected when
-// score > thr and its rank by descending score (ties: lower input index first) is < max_det; selected rows are grouped by
-// label (ascending), in score order inside a label -- exactly the per-label arrays eval.py builds.
-__global__ void __launch_bounds__(256) eval_select_kernel(const float* __restrict__ scores, const int64_t* __restrict__ labels,
-                                                          const float* __restrict__ boxes, int n, float scale, float thr,
-                                                          int max_det, int num_classes, float* __restrict__ out_dets,
-                                                          int32_t* __restrict__ out_labels, int32_t* __restrict__ class_off,
-                                                          int32_t* __restrict__ count) {
-    extern __shared__ int32_t sm[];
-    int32_t* sel = sm;                    // [max_det] input index of the detection with rank r
-    int32_t* cls_cnt = sm + max_det;      // [num_classes + 1]
-    __shared__ int nsel;
-    for (int i = threadIdx.x; i < max_det; i += blockDim.x) sel[i] = -1;
-    for (int i = threadIdx.x; i <= num_classes; i += blockDim.x) cls_cnt[i] = 0;
-    if (threadIdx.x == 0) nsel = 0;
-    __syncthreads();
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const float s = scores[i];
-        if (!(s > thr)) continue;
-        int rank = 0;
-        for (int j = 0; j < n; ++j) {
-            const float t = scores[j];
-            rank += (t > thr) && (t > s || (t == s && j < i));
-        }
-        if (rank < max_det) {
-            sel[rank] = i;
-            atomicAdd(&nsel, 1);
-        }
-    }
-    __syncthreads();
-    const int m = nsel;
-    for (int r = threadIdx.x; r < m; r += blockDim.x) {
-        const int lab = (int)labels[sel[r]];
-        if (lab >= 0 && lab < num_classes) atomicAdd(&cls_cnt[lab + 1], 1);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int c = 0; c < num_classes; ++c) cls_cnt[c + 1] += cls_cnt[c];
-        count[0] = m;
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c <= num_classes; c += blockDim.x) class_off[c] = cls_cnt[c];
-    // stable placement: position of rank r inside its label group = number of lower ranks with the same label
-    for (int r = threadIdx.x; r < m; r += blockDim.x) {
-        const int i = sel[r];
-        const int lab = (int)labels[i];
-        if (lab < 0 || lab >= num_classes) continue;
-        int pos = 0;
-        for (int q = 0; q < r; ++q) pos += ((int)labels[sel[q]] == lab);
-        const int dst = cls_cnt[lab] + pos;
-        const float4 bx = *reinterpret_cast<const float4*>(boxes + (long long)i * 4);
-        float* o = out_dets + (long long)dst * 5;
-        o[0] = __fdiv_rn(bx.x, scale);                                // boxes /= scale   (float32 array / float32 scalar)
-        o[1] = __fdiv_rn(bx.y, scale);
-        o[2] = __fdiv_rn(bx.z, scale);
-        o[3] = __fdiv_rn(bx.w, scale);
-        o[4] = scores[i];
-        out_labels[dst] = lab;
-    }
-}
-
 }  // namespace effdet
 
 using namespace effdet;
@@ -149,19 +88,4 @@ extern "C" int effdet_collate_annots(const double* rows, const int32_t* row_off,
     EFFDET_DEVICE(device);
     collate_annots_kernel<<<cdiv((long long)B * G, 128), 128, 0, (cudaStream_t)stream>>>(rows, row_off, scale, flip, width, out, B, G);
     return launch_status("collate_annots_kernel");
-}
-
-extern "C" int effdet_eval_select(const float* scores, const int64_t* labels, const float* boxes, int n, float scale,
-                                  float score_threshold, int max_det, int num_classes, float* out_dets, int32_t* out_labels,
-                                  int32_t* class_offsets, int32_t* count, int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(out_dets && out_labels && class_offsets && count && n >= 0 && max_det > 0 && num_classes > 0 &&
-                       (n == 0 || (scores && labels && boxes)),
-                   "eval_select: bad arguments");
-    EFFDET_REQUIRE((size_t)(max_det + num_classes + 1) * 4 <= 48 * 1024, "eval_select: max_det + num_classes too large");
-    EFFDET_REQUIRE(aligned16(boxes), "eval_select: boxes must be 16-byte aligned");
-    EFFDET_REQUIRE(scale > 0.f, "eval_select: scale must be positive");
-    EFFDET_DEVICE(device);
-    eval_select_kernel<<<1, 256, (size_t)(max_det + num_classes + 1) * 4, (cudaStream_t)stream>>>(
-        scores, labels, boxes, n, scale, score_threshold, max_det, num_classes, out_dets, out_labels, class_offsets, count);
-    return launch_status("eval_select_kernel");
 }

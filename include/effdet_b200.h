@@ -410,6 +410,42 @@ int effdet_eval_select(const float* scores, const int64_t* labels, const float* 
                        int32_t* class_offsets, int32_t* count, int device, effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * VOC mean average precision on the device (eval.py::evaluate, eval.py:165-257), for a whole test set without a host
+ * read until the end.  A record is one detection slot: image i owns records i*max_det .. (i+1)*max_det - 1.
+ *
+ * effdet_eval_select_batch: effdet_eval_select for B images at once, on the padded output of the batched detection
+ *   (scores [B,C], labels [B,C] int64, boxes [B,C,4] 16-byte aligned, count [B] int32 kept rows, -1 = NMS overflow),
+ *   with per-image scales scale [B] float on the device.  Image b's rows equal effdet_eval_select(..., count[b],
+ *   scale[b], ...) bit for bit and go to out_dets [B][max_det][5], out_labels [B][max_det] (-1: empty slot) and
+ *   class_offsets [B][num_classes+1].  count[b] == -1: every label -1 and overflow[b] = 1 (else 0).
+ *   score_threshold >= 0 (the AP key below relies on positive scores).
+ * effdet_voc_match: eval.py:199-224 for the B images of one effdet_eval_select_batch call.  Ground truth: gt [num_gt,5]
+ *   fp64 rows (x1,y1,x2,y2,label) in original image coordinates, image b owns rows gt_offsets[b] .. gt_offsets[b+1]
+ *   ([B+1] int32 on the device).  Per (image, class) the detections are taken in slot order (score descending) and
+ *   matched greedily: IoU as compute_overlap computes it (fp64, no FMA contraction), the first maximum wins, TP iff
+ *   IoU >= iou_threshold and that ground truth is not taken yet.  tp [B][max_det] uint8 = 1 (TP) / 0 (FP) for every
+ *   filled slot; gt_count [num_classes] int64 += ground-truth rows per class.
+ * effdet_voc_ap: eval.py:226-248 for every class over num_records records (dets [R][5], labels [R], tp [R] as written
+ *   above, gt_count as accumulated above) -> ap [num_classes] fp64, num_annotations [num_classes] fp64 (both 0 for a
+ *   class without ground truth).  Records of one class are ordered by score descending, ties by record index (image,
+ *   then rank inside the image): the order a stable sort of the reference's append order gives.  Sums follow NumPy's
+ *   pairwise summation, so the results equal the reference's float64 values.  The sort key packs class (8 bits),
+ *   score (31 bits) and record index (25 bits): num_classes <= 255 and num_records <= 2^25 (33,554,432).
+ *   workspace: effdet_voc_ap_workspace(num_records, num_classes) bytes, 16-byte aligned (-1 when over the limits).
+ * ------------------------------------------------------------------------------------------ */
+int effdet_eval_select_batch(const float* scores, const int64_t* labels, const float* boxes, const int32_t* count,
+                             const float* scale, int B, int C, float score_threshold, int max_det, int num_classes,
+                             float* out_dets, int32_t* out_labels, int32_t* class_offsets, int32_t* overflow, int device,
+                             effdet_stream_t stream);
+int effdet_voc_match(const float* dets, const int32_t* class_offsets, const double* gt, const int32_t* gt_offsets,
+                     int num_gt, int B, int max_det, int num_classes, double iou_threshold, uint8_t* tp,
+                     int64_t* gt_count, int device, effdet_stream_t stream);
+int64_t effdet_voc_ap_workspace(int num_records, int num_classes);
+int effdet_voc_ap(const float* dets, const int32_t* labels, const uint8_t* tp, const int64_t* gt_count, int num_records,
+                  int num_classes, double* ap, double* num_annotations, void* workspace, int64_t workspace_bytes,
+                  int device, effdet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Layout plumbing at the module boundary (callers see logical NCHW, kernels are NHWC).
  * ------------------------------------------------------------------------------------------ */
 int effdet_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, int device, effdet_stream_t stream);
