@@ -389,8 +389,8 @@ int effdet_multi_clip_adamw_dev(const uint64_t* p_ptrs, const uint64_t* g_ptrs, 
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) rank 2: the step BEFORE the hot path, on the device.  Normalizer + Augmenter (horizontal flip) + zero pad
  * to the common size + collater + `.cuda().float()` (datasets/augmentation.py:69-91,111-150, train.py:105-106), bit-identical
- * to NumPy: (float32(u8) - mean) / std evaluated in float64, then cast to float32.  cv2.resize is not reproduced: images
- * enter at their final resolution (h, w <= S).
+ * to NumPy: (float32(u8) - mean) / std evaluated in float64, then cast to float32.  effdet_normalize_pad takes images at
+ * their final resolution (h, w <= S); effdet_resize_normalize_pad below also runs Resizer's cv2.resize.
  *   pixels  : uint8 HWC images back to back, image b starts at byte offsets[b] and is hw[2b] x hw[2b+1] x 3
  *   flip    : [B] or NULL;  out_nchw : float32 [B,3,S,S];  mean3 / std3 : 3 host doubles
  *   annotations: rows [sum n_b, 5] float64, image b owns rows row_off[b] .. row_off[b+1]; out float32 [B,G,5], -1 padded;
@@ -401,6 +401,14 @@ int effdet_normalize_pad(const uint8_t* pixels, const int64_t* offsets, const in
                          effdet_stream_t stream);
 int effdet_collate_annots(const double* rows, const int32_t* row_off, const double* scale, const uint8_t* flip,
                           const int32_t* width, float* out, int B, int G, int device, effdet_stream_t stream);
+/* The same input step with Resizer's cv2.resize (datasets/augmentation.py:94-115,118-150): images of any size h, w >= 1,
+ * image b resized (after the flip) to resized_hw[2b] x resized_hw[2b+1] (1 .. S each) by OpenCV's generic INTER_LINEAR
+ * for CV_64FC3 on the float64 normalized image, zero padded to S x S, cast to float32 once.  pixel_scale selects the
+ * Normalizer's input: 1 = float32(u8) (COCO), 255 = float32(u8) / 255.f (VOC, datasets/voc0712.py:109).  Offsets, hw
+ * and flip as effdet_normalize_pad; the annotations go through effdet_collate_annots with Resizer's scale. */
+int effdet_resize_normalize_pad(const uint8_t* pixels, const int64_t* offsets, const int32_t* hw, const int32_t* resized_hw,
+                                const uint8_t* flip, float* out_nchw, int B, int S, int pixel_scale, const double* mean3,
+                                const double* std3, int device, effdet_stream_t stream);
 /* SURVEY.md 8(f) rank 3: the step AFTER NMS (eval.py:105-128) for one image: boxes /= scale, score > threshold,
  * top-max_det by score (ties: lower input index), split per label.  out_dets [max_det,5] (x1,y1,x2,y2,score) grouped by
  * label ascending and in score order inside a label, out_labels [max_det], class_offsets [num_classes+1] (rows of label c
