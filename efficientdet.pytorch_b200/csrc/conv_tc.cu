@@ -32,10 +32,8 @@ constexpr int kTcThreads = 288;        // two gather / MMA / epilogue warpgroups
 constexpr int kTcProducers = 256;      // the two warpgroups (all of the gathering weight-gradient kernel)
 constexpr int kTileM = 128;     // pixels per CTA (fwd/dgrad) or output channels per CTA (wgrad)
 constexpr int kTileK = 64;      // bf16 elements per 128-byte swizzled row
-// Most pixel chunks (<= 64 pixels each) one weight-gradient CTA accumulates in its wgmma fp32 accumulator.  That
-// accumulation's error grows linearly with the K steps it covers (H100, bf16x3, whole-tensor norm-relative: 4.5e-6 at
-// <= 12 chunks, 1.0e-5 at 43, 1.9e-5 at 86, 3.8e-5 at 171), so long K ranges are split further and added by atomics.
-constexpr int kWgMaxChunksPerSplit = 64;
+// Most pixel chunks (<= 64 pixels each) one weight-gradient CTA accumulates (kWgMaxPixelsPerSplit, tc_ptx.cuh).
+constexpr int kWgMaxChunksPerSplit = kWgMaxPixelsPerSplit / kTileK;
 
 // ---------------------------------------------------------------------------------------------
 // forward / data-gradient kernel

@@ -401,7 +401,8 @@ static size_t dw_bwd_smem() {
                     (K * K + 4) * (kDwT / 32) * kCVc + 10 * kCVc) * sizeof(float4);
 }
 
-// tiles per CTA: keep >= ~6 waves of CTAs in the grid, but let a CTA amortise its reductions over up to 8 tiles
+// tiles per CTA: keep >= ~6 waves of CTAs in the grid, but let a CTA amortise its reductions over up to 8 tiles.
+// tests/test_benchmark_plans.py (_dw_plan) mirrors this and the tile grids of both launchers.
 static int pick_tiles_per_cta(long long ntiles, long long other) {
     long long tpc = (ntiles * other) / (148ll * 6 * 3);
     if (tpc < 1) tpc = 1;

@@ -254,8 +254,12 @@ int pw_wgrad_launch(const effdet_wgrad_args* a, cudaStream_t st) {
     while (P.K > 16 && P.K * octs > capacity) P.K >>= 1;
     if (P.K * octs > capacity) return fail(EFFDET_ERR_UNSUPPORTED, "wgrad(pw): tile does not fit");   // (octs <= 32: 16 * 32 = 512 always fits)
     P.nchunks = cdiv(P.M, P.K);
+    // split-K: one wave of CTAs, more when a CTA would accumulate more than kWgMaxPixelsPerSplit pixels (then whole
+    // waves).  tests/test_benchmark_plans.py (_pw_plan) mirrors this arithmetic.
     int splits = num_sms() / tiles;
     if (splits < 1) splits = 1;
+    const int need = cdiv(P.nchunks, kWgMaxPixelsPerSplit / P.K);
+    if (splits < need) splits = cdiv(need * tiles, num_sms()) * num_sms() / tiles;
     if (splits > P.nchunks) splits = P.nchunks;
     P.cps = cdiv(P.nchunks, splits);
     splits = cdiv(P.nchunks, P.cps);

@@ -222,6 +222,7 @@ extern "C" int effdet_stem_wgrad(const float* x_nchw, const float* dz, float* dw
     EFFDET_REQUIRE(aligned16(dz), "stem_wgrad: alignment");
     EFFDET_DEVICE(device);
     const int Ho = (H + 1 - 3) / 2 + 1, Wo = (W + 1 - 3) / 2 + 1;
+    // grid and TPG: tests/test_benchmark_plans.py (_stem_plan) mirrors this arithmetic
     const int segs = cdiv(Wo, kStemP);
     const long long units = (long long)B * Ho * segs;
     int blocks = (int)(units < num_sms() * 8 ? units : num_sms() * 8);

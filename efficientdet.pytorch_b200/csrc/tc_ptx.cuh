@@ -10,6 +10,12 @@
 
 namespace effdet {
 
+// Most pixels (GEMM-K) one weight-gradient CTA accumulates in its wgmma fp32 accumulator: 64 chunks of 64 pixels.  That
+// accumulation's error grows linearly with the K range it covers (H100, bf16x3, whole-tensor norm-relative: 4.5e-6 at
+// <= 768 pixels, 1.0e-5 at 2 752, 1.9e-5 at 5 504, 3.8e-5 at 10 944), so longer ranges are split further and added by
+// atomics.  Both weight-gradient launchers read it: conv_tc.cu and pw_wgrad.cu.
+constexpr int kWgMaxPixelsPerSplit = 4096;
+
 // ---------------------------------------------------------------------------------------------
 // PTX wrappers
 // ---------------------------------------------------------------------------------------------
