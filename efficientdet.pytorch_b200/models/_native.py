@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.normpath(os.path.join(_HERE, '..', 'csrc'))
 SO_PATH = os.path.join(CSRC, 'libeffdet_b200.so')
 SOURCES = ['api.cu', 'conv_api.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_planes.cu', 'pw_gemm.cu', 'pw_wgrad.cu', 'stem.cu', 'dw_fused.cu', 'mbconv_ops.cu', 'se_ops.cu', 'bifpn.cu', 'pipeline.cu',
-           'loss.cu', 'detect.cu', 'layout.cu', 'optim.cu', 'voc_eval.cu']
+           'loss.cu', 'detect.cu', 'layout.cu', 'optim.cu', 'voc_eval.cu', 'coco_eval.cu']
 NVCC_FLAGS = ['-std=c++17', '-O3', '-lineinfo', '-gencode', 'arch=compute_90a,code=sm_90a',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -33,6 +33,7 @@ def build(force=False, verbose=False):
     from concurrent.futures import ThreadPoolExecutor
     import hashlib
     hdrs = [os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'tc_ptx.cuh'), os.path.join(CSRC, 'bitonic.cuh'),
+            os.path.join(CSRC, 'block_scan.cuh'),
             os.path.normpath(os.path.join(CSRC, '..', '..', 'include', 'effdet_b200.h'))]
     hdr_blob = b''.join(open(h, 'rb').read() for h in hdrs if os.path.exists(h))
     nvcc = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
@@ -168,13 +169,17 @@ SIGNATURES = {
     'effdet_eval_select_batch': [_P] * 5 + [_INT, _INT, _F, _INT, _INT] + [_P] * 4 + _TAIL,
     'effdet_voc_match': [_P] * 4 + [_INT] * 4 + [ctypes.c_double, _P, _P] + _TAIL,
     'effdet_voc_ap': [_P] * 4 + [_INT, _INT] + [_P] * 3 + [_I64] + _TAIL,
+    'effdet_coco_select_batch': [_P] * 6 + [_INT, _INT, ctypes.c_double, _P] + [_INT] * 4 + [_P] * 9 + _TAIL,
+    'effdet_coco_match': [_P] * 5 + [_INT, _P, _P] + [_INT] * 3 + [_P, _INT, _INT, _P, _P] + _TAIL,
+    'effdet_coco_accumulate': [_P] * 8 + [_INT] * 4 + [_INT] * 3 + [_P] * 3 + [_I64] + _TAIL,
     'effdet_nchw_to_nhwc': [_P, _P, _INT, _INT, _INT, _INT] + _TAIL,
     'effdet_nhwc_to_nchw': [_P, _P, _INT, _INT, _INT, _INT] + _TAIL,
 }
 PLAIN = {'effdet_version': (ctypes.c_int, []), 'effdet_conv_tc_kpad': (ctypes.c_int, [ctypes.c_int]),
          'effdet_wgrad_tc_geometry_ok': (ctypes.c_int, [ctypes.c_int] * 3), 'effdet_last_error': (ctypes.c_char_p, []),
          'effdet_launch_count': (ctypes.c_uint64, []), 'effdet_reset_launch_count': (None, []),
-         'effdet_voc_ap_workspace': (ctypes.c_int64, [ctypes.c_int] * 2)}
+         'effdet_voc_ap_workspace': (ctypes.c_int64, [ctypes.c_int] * 2),
+         'effdet_coco_accumulate_workspace': (ctypes.c_int64, [ctypes.c_int] * 3)}
 
 _lib = None
 _lock = threading.Lock()

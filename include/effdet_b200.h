@@ -454,6 +454,58 @@ int effdet_voc_ap(const float* dets, const int32_t* labels, const uint8_t* tp, c
                   int device, effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * COCO box mAP on the device (eval.py::evaluate_coco, eval.py:260-338, with pycocotools' COCOeval for iouType 'bbox'
+ * and default Params), for a whole test set without a host read until the end.  Images are identified by their rank
+ * among the sorted image ids (COCOeval's imgIds), categories by their index among the sorted category ids (catIds).
+ * Records live in a buffer of `capacity` slots: rec_box [capacity] float4 (x, y, w, h after boxes /= scale, in
+ * float32), rec_score [capacity] float, rec_meta [capacity] int4 (model label, category index or -1, image rank, rank
+ * inside (image, category) after a stable sort by score descending), rec_meta initialised to -1 by the caller.
+ * Limits: num_categories <= 255, num_images <= 2^18, capacity <= 2^25, max_gt <= 256 ground truths per (image,
+ * category).
+ *
+ * effdet_coco_select_batch: eval.py:280-311 for B images of the padded detection output (scores [B,C], labels [B,C]
+ *   int64, boxes [B,C,4] 16-byte aligned, count [B] int32 kept rows, -1 = NMS overflow) with per-image scale [B]
+ *   float and image_rank [B] int32 on the device.  Image b records its rows in NMS order up to the first with
+ *   (double)score < score_threshold; label l maps to category label_category[l] (-1 when l is outside
+ *   [0, num_labels) or maps to no ground-truth category).  The rows go to the slots at the device-side cursor (int64,
+ *   records asked for so far, also past capacity), in batch order; image_offset / image_count [num_images] (indexed by
+ *   rank) and batch_offset / batch_count [B] receive each image's slots.  status [B]: 0 recorded, 1 NMS overflow
+ *   (nothing recorded), 2 out of capacity (nothing recorded).
+ * effdet_coco_match: COCOeval.computeIoU + evaluateImg for the images of one effdet_coco_select_batch call (the same
+ *   image_rank, batch_offset, batch_count).  Ground truth gt [n,6] fp64 (x, y, w, h, area, iscrowd) grouped by
+ *   (image rank, category) in annotation order: group q*num_categories + k owns rows gt_offsets[..] ..
+ *   gt_offsets[..+1] (int32 [num_images*num_categories+1]); max_gt = the largest group.  iou_thrs: the 10 fp64 values
+ *   of Params.iouThrs on the device; iou_type must be EFFDET_COCO_BBOX.  flags [capacity][4] uint32 per record of rank
+ *   < 100 and area range (all, small, medium, large): bit t = matched at threshold t, bit 16+t = ignored.
+ *   npig [num_categories][4] int64 += non-ignored ground truths.
+ * effdet_coco_accumulate: COCOeval.accumulate -> precision [10][101][num_categories][4][3] and recall
+ *   [10][num_categories][4][3] fp64 (-1 where a (category, area range) has no non-ignored ground truth).  rec_thrs: the
+ *   101 fp64 values of Params.recThrs on the device; max_dets must be (1, 10, 100).  Records of one category are
+ *   ordered by score descending, then image rank, then rank inside (image, category), with one 64-bit key sort over
+ *   category (8 bits), score (31) and the record's position in image-rank order (25).  workspace:
+ *   effdet_coco_accumulate_workspace(capacity, num_images, num_categories) bytes, 16-byte aligned.
+ * ------------------------------------------------------------------------------------------ */
+#define EFFDET_COCO_BBOX 1
+int effdet_coco_select_batch(const float* scores, const int64_t* labels, const float* boxes, const int32_t* count,
+                             const float* scale, const int32_t* image_rank, int B, int C, double score_threshold,
+                             const int32_t* label_category, int num_labels, int num_categories, int num_images,
+                             int capacity, float* rec_box, float* rec_score, int32_t* rec_meta, int64_t* cursor,
+                             int32_t* image_offset, int32_t* image_count, int32_t* status, int32_t* batch_offset,
+                             int32_t* batch_count, int device, effdet_stream_t stream);
+int effdet_coco_match(const float* rec_box, const int32_t* rec_meta, const int32_t* batch_offset,
+                      const int32_t* batch_count, const int32_t* image_rank, int B, const double* gt,
+                      const int32_t* gt_offsets, int num_images, int num_categories, int max_gt, const double* iou_thrs,
+                      int num_iou_thrs, int iou_type, uint32_t* flags, int64_t* npig, int device,
+                      effdet_stream_t stream);
+int64_t effdet_coco_accumulate_workspace(int capacity, int num_images, int num_categories);
+int effdet_coco_accumulate(const float* rec_score, const int32_t* rec_meta, const uint32_t* flags,
+                           const int64_t* cursor, const int32_t* image_offset, const int32_t* image_count,
+                           const int64_t* npig, const double* rec_thrs, int num_rec_thrs, int max_det0, int max_det1,
+                           int max_det2, int capacity, int num_images, int num_categories, double* precision,
+                           double* recall, void* workspace, int64_t workspace_bytes, int device,
+                           effdet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Layout plumbing at the module boundary (callers see logical NCHW, kernels are NHWC).
  * ------------------------------------------------------------------------------------------ */
 int effdet_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, int device, effdet_stream_t stream);
