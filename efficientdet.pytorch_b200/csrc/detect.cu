@@ -138,22 +138,78 @@ __device__ __forceinline__ bool iou_gt(const float4 a, const float4 b, double th
     return (double)ovr > thr;
 }
 
-// Candidates NMS works on in image b: count[b], or 0 when count[b] > cap (overflow).
-__device__ __forceinline__ int nms_candidates(const int32_t* count, int b, int cap) {
+// Greedy NMS in column chunks of `chunk` sorted candidates.  Chunk c of image b covers its sorted candidates
+// [base, base + chunk) with base = c * chunk.  Candidate j is kept iff no kept i < j has IoU > thr: the cross step decides
+// that against the boxes kept by earlier chunks, the mask + scan inside the chunk.  Every kernel calls
+// iou_gt(earlier box, later box), so the keep set and its order do not depend on `chunk`.  With chunk = cap there is one
+// chunk and no cross step: the mask + scan over all candidates.
+//
+// Candidates of image b inside the chunk at `base`: 0 when count[b] > cap (overflow) or when the image ends before it.
+__device__ __forceinline__ int nms_candidates(const int32_t* count, int b, int cap, int base, int chunk) {
     const int n = count[b];
-    return n > cap ? 0 : n;
+    return n > cap || n <= base ? 0 : min(n - base, chunk);
 }
 
-// Persistent over the upper-triangle 64x64 tiles of all B images, numbered image by image and row by row inside an
-// image (row rb holds tiles cb = rb .. cw_b-1, cw_b = ceil(n_b/64)).  The grid depends on B and cap only.  Each CTA
-// walks that numbering forward as its tile index grows, so the walk costs O(B + rows) per CTA in total.
-// mask[b][i][cb] bit j set  <=>  sorted box (64*cb + j) of image b is suppressed by its sorted box i; row stride ceil(cap/64).
+constexpr int kCrossThreads = 256;
+
+// Cross step of the chunk at `base` > 0.  CTA (x, y, b) tests the 64 candidates of tile y against every gridDim.x-th
+// tile of kCrossThreads boxes among the nkeep[b] that image b kept in earlier chunks (read through keep_idx, one kept box
+// per thread) and ORs the candidates they suppress into removed[b][y].  A candidate already removed is not tested again,
+// and a CTA stops once its whole tile is removed.  removed[b] is zero on entry: the scan of the previous chunk cleared it.
+__global__ void __launch_bounds__(kCrossThreads) nms_cross_kernel(const float* __restrict__ boxes,
+                                                                  const uint64_t* __restrict__ keys,
+                                                                  const int32_t* __restrict__ count, int A, int npad,
+                                                                  int cap, int base, int chunk, double thr,
+                                                                  const int32_t* __restrict__ keep_idx,
+                                                                  const int32_t* __restrict__ nkeep, uint64_t* removed) {
+    __shared__ float4 cbx[64];
+    __shared__ uint64_t done;
+    const int b = blockIdx.z;
+    const int valid = min(64, nms_candidates(count, b, cap, base, chunk) - (int)blockIdx.y * 64);
+    if (valid <= 0) return;
+    const uint64_t valid_bits = valid == 64 ? ~0ull : (1ull << valid) - 1ull;
+    const float* bx = boxes + (long long)b * A * 4;
+    if (threadIdx.x < valid)
+        cbx[threadIdx.x] = ldg4(bx + (long long)(uint32_t)keys[(long long)b * npad + base + blockIdx.y * 64 + threadIdx.x] * 4);
+    uint64_t* word = removed + (long long)b * ((chunk + 63) / 64) + blockIdx.y;
+    const int nk = nkeep[b];
+    keep_idx += (long long)b * cap;
+    for (int k0 = blockIdx.x * kCrossThreads; k0 < nk; k0 += gridDim.x * kCrossThreads) {
+        __syncthreads();                       // cbx is stored, and every thread has read the previous `done`
+        if (threadIdx.x == 0) done = *(volatile uint64_t*)word;
+        __syncthreads();
+        const uint64_t live = ~done & valid_bits;
+        if (!live) break;
+        uint64_t bits = 0;
+        const int k = k0 + threadIdx.x;
+        if (k < nk) {
+            const float4 me = ldg4(bx + (long long)keep_idx[k] * 4);
+            for (uint64_t m = live; m; m &= m - 1) {          // CTA-uniform: no divergence from the removed bits
+                const int j = __ffsll((long long)m) - 1;
+                if (iou_gt(me, cbx[j], thr)) bits |= 1ull << j;
+            }
+        }
+        const uint32_t lo = __reduce_or_sync(0xffffffffu, (uint32_t)bits);
+        const uint32_t hi = __reduce_or_sync(0xffffffffu, (uint32_t)(bits >> 32));
+        if ((threadIdx.x & 31) == 0 && (lo | hi))
+            atomicOr((unsigned long long*)word, ((unsigned long long)hi << 32) | lo);
+    }
+}
+
+// Persistent over the upper-triangle 64x64 tiles of the chunk at `base` in all B images, numbered image by image and row
+// by row inside an image (row rb holds tiles cb = rb .. cw_b-1, cw_b = ceil(n_b/64), n_b the image's candidates in the
+// chunk).  The grid depends on B and chunk only.  Each CTA walks that numbering forward as its tile index grows, so the
+// walk costs O(B + rows) per CTA in total.
+// mask[b][i][cb] bit j set  <=>  sorted box base + 64*cb + j of image b is suppressed by its sorted box base + i; row
+// stride ceil(chunk/64).  removed (null for the first chunk): the cross step's bitmap.  A row whose candidate it removed
+// is written as zero without testing, because the scan never uses that row.
 __global__ void __launch_bounds__(64) nms_mask_kernel(const float* __restrict__ boxes, const uint64_t* __restrict__ keys,
                                                       const int32_t* __restrict__ count, int B, int A, int npad, int cap,
-                                                      double thr, uint64_t* __restrict__ mask) {
+                                                      int base, int chunk, double thr, const uint64_t* __restrict__ removed,
+                                                      uint64_t* __restrict__ mask) {
     __shared__ float4 cbx[64];
-    const int cw_cap = (cap + 63) / 64;
-    int b = 0, n = nms_candidates(count, 0, cap), cw = (n + 63) / 64;
+    const int cw_chunk = (chunk + 63) / 64;
+    int b = 0, n = nms_candidates(count, 0, cap, base, chunk), cw = (n + 63) / 64;
     long long img_base = 0, img_tiles = (long long)cw * (cw + 1) / 2;   // first tile of image b, tiles of image b
     int rb = 0;
     long long row_base = 0;                                            // first tile of row rb, relative to img_base
@@ -161,7 +217,7 @@ __global__ void __launch_bounds__(64) nms_mask_kernel(const float* __restrict__ 
         while (t >= img_base + img_tiles) {
             img_base += img_tiles;
             if (++b >= B) return;
-            n = nms_candidates(count, b, cap);
+            n = nms_candidates(count, b, cap, base, chunk);
             cw = (n + 63) / 64;
             img_tiles = (long long)cw * (cw + 1) / 2;
             rb = 0;
@@ -173,7 +229,7 @@ __global__ void __launch_bounds__(64) nms_mask_kernel(const float* __restrict__ 
             ++rb;
         }
         const int cb = rb + (int)(local - row_base);
-        const uint64_t* kb = keys + (long long)b * npad;
+        const uint64_t* kb = keys + (long long)b * npad + base;
         const float* bx = boxes + (long long)b * A * 4;
         const int cj = cb * 64 + threadIdx.x;
         if (cj < n) cbx[threadIdx.x] = ldg4(bx + (long long)(uint32_t)kb[cj] * 4);
@@ -183,7 +239,9 @@ __global__ void __launch_bounds__(64) nms_mask_kernel(const float* __restrict__ 
             const float4 me = ldg4(bx + (long long)(uint32_t)kb[i] * 4);
             const int csize = min(64, n - cb * 64);
             uint64_t bits = 0;
-            if (rb != cb && csize == 64) {             // almost every tile: fixed trip count, constant bit positions
+            if (removed && ((removed[(long long)b * cw_chunk + rb] >> threadIdx.x) & 1ull)) {
+                // suppressed by a box of an earlier chunk
+            } else if (rb != cb && csize == 64) {      // almost every tile: fixed trip count, constant bit positions
 #pragma unroll 8
                 for (int j = 0; j < 64; ++j)
                     if (iou_gt(me, cbx[j], thr)) bits |= 1ull << j;
@@ -191,43 +249,57 @@ __global__ void __launch_bounds__(64) nms_mask_kernel(const float* __restrict__ 
                 for (int j = (rb == cb ? threadIdx.x + 1 : 0); j < csize; ++j)
                     if (iou_gt(me, cbx[j], thr)) bits |= 1ull << j;
             }
-            mask[((long long)b * cap + i) * cw_cap + cb] = bits;
+            mask[((long long)b * chunk + i) * cw_chunk + cb] = bits;
         }
         __syncthreads();
     }
 }
 
-// Greedy scan over the sorted candidates, one CTA per image; the `removed` bitmap lives in shared memory.  Candidates are
-// consumed 64 at a time: warp 0 resolves the block's internal dependencies from the 64 diagonal mask words (a
-// sequential walk over 64 bits, registers + shuffles only), then every thread ORs the rows of the block's survivors
-// into its slice of `removed`.  Two CTA barriers per 64 candidates instead of two per kept box: the scan used to be
-// 255 ms for the 55 k survivors of a random-weight D7 image.  Result identical to the one-at-a-time scan.
+// Greedy scan over the sorted candidates of the chunk at `base`, one CTA per image; the `removed` bitmap lives in shared
+// memory.  Candidates are consumed 64 at a time: warp 0 resolves the block's internal dependencies from the 64 diagonal
+// mask words (a sequential walk over 64 bits, registers + shuffles only), then every thread ORs the rows of the block's
+// survivors into its slice of `removed`.  Two CTA barriers per 64 candidates instead of two per kept box: the scan used
+// to be 255 ms for the 55 k survivors of a random-weight D7 image.  Result identical to the one-at-a-time scan.
+// The first chunk starts from an empty bitmap and keep list; a later one starts from the cross step's bitmap
+// removed_g[b] and appends at keep_idx[b][nkeep[b]].  The scan clears removed_g[b] for the next chunk's cross step;
+// removed_g is null when there is one chunk.
 // nkeep[b] = kept boxes, or -1 when count[b] > cap (nothing else is written for that image).
 __global__ void __launch_bounds__(1024) nms_scan_kernel(const uint64_t* __restrict__ mask, const uint64_t* __restrict__ keys,
-                                                        const int32_t* __restrict__ count, int npad, int cap,
+                                                        const int32_t* __restrict__ count, int npad, int cap, int base,
+                                                        int chunk, uint64_t* __restrict__ removed_g,
                                                         int32_t* __restrict__ keep_idx, int32_t* __restrict__ nkeep) {
     extern __shared__ uint64_t removed[];
     __shared__ uint64_t keep_bits;
     const int b = blockIdx.x;
-    const int n = count[b];
-    if (n > cap) {
-        if (threadIdx.x == 0) nkeep[b] = -1;
+    const int total = count[b];
+    if (total > cap) {
+        if (threadIdx.x == 0 && base == 0) nkeep[b] = -1;
         return;
     }
-    const int cw_cap = (cap + 63) / 64;
-    mask += (long long)b * cap * cw_cap;
-    keys += (long long)b * npad;
+    if (base > 0 && total <= base) return;                          // the image ended in an earlier chunk
+    const int n = min(total - base, chunk);
+    const int cw_chunk = (chunk + 63) / 64;
+    mask += (long long)b * chunk * cw_chunk;
+    keys += (long long)b * npad + base;
     keep_idx += (long long)b * cap;
     const int col_blocks = (n + 63) / 64;
     const int lane = threadIdx.x & 31;
-    for (int j = threadIdx.x; j < col_blocks; j += blockDim.x) removed[j] = 0;
+    int kept = base > 0 ? nkeep[b] : 0;
+    for (int j = threadIdx.x; j < col_blocks; j += blockDim.x) {
+        uint64_t r = 0;
+        if (removed_g) {
+            uint64_t* w = removed_g + (long long)b * cw_chunk + j;
+            if (base > 0) r = *w;
+            *w = 0;
+        }
+        removed[j] = r;
+    }
     __syncthreads();
-    int kept = 0;
     for (int nb = 0; nb < col_blocks; ++nb) {
         if (threadIdx.x < 32) {
             const int i0 = nb * 64 + lane, i1 = i0 + 32;
-            const uint64_t d0 = i0 < n ? mask[(long long)i0 * cw_cap + nb] : 0ull;     // bits j > i inside the block
-            const uint64_t d1 = i1 < n ? mask[(long long)i1 * cw_cap + nb] : 0ull;
+            const uint64_t d0 = i0 < n ? mask[(long long)i0 * cw_chunk + nb] : 0ull;   // bits j > i inside the block
+            const uint64_t d1 = i1 < n ? mask[(long long)i1 * cw_chunk + nb] : 0ull;
             uint64_t rem = removed[nb], kb = 0;
             const int valid = min(64, n - nb * 64);
 #pragma unroll 1
@@ -249,7 +321,7 @@ __global__ void __launch_bounds__(1024) nms_scan_kernel(const uint64_t* __restri
             while (bits) {
                 const int bit = __ffsll((long long)bits) - 1;
                 bits &= bits - 1;
-                acc |= mask[(long long)(nb * 64 + bit) * cw_cap + j];
+                acc |= mask[(long long)(nb * 64 + bit) * cw_chunk + j];
             }
             removed[j] |= acc;
         }
@@ -313,21 +385,49 @@ int bitonic_sort_launch(uint64_t* keys, int n, int seg, cudaStream_t st) {
     return EFFDET_OK;
 }
 
+// Workspace of the chunked NMS: the chunk's mask [B][chunk][ceil(chunk/64)], then (more than one chunk) the cross step's
+// bitmaps [B][ceil(chunk/64)].  With one chunk this is effdet_nms_batch's mask [B][cap][ceil(cap/64)].
+static long long nms_workspace_words(int B, int cap, int chunk) {
+    const long long cw = cdiv(chunk, 64);
+    return (long long)B * (chunk * cw + (cdiv(cap, chunk) > 1 ? cw : 0));
+}
+
+// ceil(cap/chunk) chunks, each a fixed set of launches (cross step from the second chunk on, mask, scan): the sequence
+// depends on B, cap and chunk only, so it can be captured.  Launches for a chunk past an image's count exit at once.
 static int nms_launch(const float* boxes, const uint64_t* keys, const int32_t* count, int B, int A, int npad, int cap,
-                      double iou_threshold, uint64_t* mask_ws, int32_t* keep_idx, int32_t* nkeep, cudaStream_t st) {
-    const long long cw = cdiv(cap, 64);
-    const long long tiles = (long long)B * (cw * (cw + 1) / 2);        // upper bound: every image at `cap` candidates
-    const int grid = (int)(tiles < (long long)num_sms() * 32 ? tiles : (long long)num_sms() * 32);
-    nms_mask_kernel<<<grid, 64, 0, st>>>(boxes, keys, count, B, A, npad, cap, iou_threshold, mask_ws);
-    int s = launch_status("nms_mask_kernel");
-    if (s) return s;
+                      int chunk, double iou_threshold, uint64_t* ws, int32_t* keep_idx, int32_t* nkeep, cudaStream_t st) {
+    const long long cw = cdiv(chunk, 64);
+    const int chunks = cdiv(cap, chunk);
+    uint64_t* mask = ws;
+    uint64_t* removed = chunks > 1 ? ws + (long long)B * chunk * cw : nullptr;
+    const long long tiles = (long long)B * (cw * (cw + 1) / 2);        // upper bound: every image at `chunk` candidates
+    const int mask_grid = (int)(tiles < (long long)num_sms() * 32 ? tiles : (long long)num_sms() * 32);
     const size_t smem = (size_t)cw * sizeof(uint64_t);
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "nms: smem opt-in: %s", cudaGetErrorString(e));
     }
-    nms_scan_kernel<<<B, 1024, smem, st>>>(mask_ws, keys, count, npad, cap, keep_idx, nkeep);
-    return launch_status("nms_scan_kernel");
+    int s;
+    for (int c = 0; c < chunks; ++c) {
+        const int base = c * chunk;
+        if (c > 0) {
+            // kept boxes before this chunk: at most `base`.  Enough CTAs along the kept list to fill the SMs about once
+            // with the (candidate tile, image) pairs; each strides over the kept tiles.
+            const int kept_tiles = cdiv(base, kCrossThreads);
+            const int fill = cdiv((long long)num_sms() * (2048 / kCrossThreads), cw * B);
+            const int gx = kept_tiles < fill ? kept_tiles : fill;
+            nms_cross_kernel<<<dim3(gx, (unsigned)cw, B), kCrossThreads, 0, st>>>(boxes, keys, count, A, npad, cap, base,
+                                                                                 chunk, iou_threshold, keep_idx, nkeep,
+                                                                                 removed);
+            if ((s = launch_status("nms_cross_kernel"))) return s;
+        }
+        nms_mask_kernel<<<mask_grid, 64, 0, st>>>(boxes, keys, count, B, A, npad, cap, base, chunk, iou_threshold,
+                                                  c > 0 ? removed : nullptr, mask);
+        if ((s = launch_status("nms_mask_kernel"))) return s;
+        nms_scan_kernel<<<B, 1024, smem, st>>>(mask, keys, count, npad, cap, base, chunk, removed, keep_idx, nkeep);
+        if ((s = launch_status("nms_scan_kernel"))) return s;
+    }
+    return EFFDET_OK;
 }
 
 static int gather_launch(const float* boxes, const float* scores, const int32_t* classes, const int32_t* keep_idx,
@@ -369,7 +469,40 @@ extern "C" int effdet_nms_batch(const float* boxes, const uint64_t* keys, const 
                    "nms_batch: cap=%d is too large for the scan bitmap (%zu bytes of shared memory at most)", cap, kScanSmemLimit);
     EFFDET_REQUIRE(aligned16(boxes), "nms_batch: alignment");
     EFFDET_DEVICE(device);
-    return nms_launch(boxes, keys, count, B, A, npad, cap, iou_threshold, mask_ws, keep_idx, nkeep, (cudaStream_t)stream);
+    return nms_launch(boxes, keys, count, B, A, npad, cap, cap, iou_threshold, mask_ws, keep_idx, nkeep,
+                      (cudaStream_t)stream);
+}
+
+#define NMS_CHUNK_LIMITS(fn, B, cap, chunk)                                                                             \
+    EFFDET_REQUIRE((B) >= 1 && (B) <= 65535, fn ": B=%d must be in [1, 65535]", (B));                                   \
+    EFFDET_REQUIRE((cap) >= 1, fn ": cap=%d must be >= 1", (cap));                                                      \
+    EFFDET_REQUIRE((chunk) >= 1 && (chunk) <= (cap) && ((chunk) % 64 == 0 || (chunk) == (cap)),                         \
+                   fn ": chunk=%d must be a multiple of 64 in [64, cap=%d], or cap itself", (chunk), (cap));            \
+    EFFDET_REQUIRE((size_t)cdiv((chunk), 64) * sizeof(uint64_t) <= kScanSmemLimit,                                      \
+                   fn ": chunk=%d is too large for the scan bitmap (%zu bytes of shared memory at most)", (chunk),      \
+                   kScanSmemLimit)
+
+extern "C" int64_t effdet_nms_chunked_workspace(int B, int cap, int chunk) {
+    NMS_CHUNK_LIMITS("nms_chunked_workspace", B, cap, chunk);
+    return nms_workspace_words(B, cap, chunk) * (int64_t)sizeof(uint64_t);
+}
+
+extern "C" int effdet_nms_batch_chunked(const float* boxes, const uint64_t* keys, const int32_t* count, int B, int A,
+                                        int npad, int cap, int chunk, double iou_threshold, void* workspace,
+                                        int64_t workspace_bytes, int32_t* keep_idx, int32_t* nkeep, int device,
+                                        effdet_stream_t stream) {
+    EFFDET_REQUIRE(boxes && keys && count && workspace && keep_idx && nkeep, "nms_batch_chunked: null tensor");
+    NMS_CHUNK_LIMITS("nms_batch_chunked", B, cap, chunk);
+    EFFDET_REQUIRE(A > 0 && npad >= A && (npad & (npad - 1)) == 0,
+                   "nms_batch_chunked: npad=%d must be a power of two >= A=%d", npad, A);
+    EFFDET_REQUIRE(cap <= A, "nms_batch_chunked: cap=%d must be in [1, A=%d]", cap, A);
+    const long long need = nms_workspace_words(B, cap, chunk) * (long long)sizeof(uint64_t);
+    EFFDET_REQUIRE(workspace_bytes >= need, "nms_batch_chunked: workspace of %lld bytes, %lld needed",
+                   (long long)workspace_bytes, need);
+    EFFDET_REQUIRE(aligned16(boxes) && aligned16(workspace), "nms_batch_chunked: boxes and workspace must be 16-byte aligned");
+    EFFDET_DEVICE(device);
+    return nms_launch(boxes, keys, count, B, A, npad, cap, chunk, iou_threshold, (uint64_t*)workspace, keep_idx, nkeep,
+                      (cudaStream_t)stream);
 }
 
 extern "C" int effdet_gather_detections_batch(const float* boxes, const float* scores, const int32_t* classes,

@@ -157,6 +157,7 @@ SIGNATURES = {
     'effdet_sigmoid_bwd': [_P, _P, _P, _I64] + _TAIL,
     'effdet_detect_candidates_batch': [_P] * 8 + [_INT, _INT, _INT, _INT, _F, _F, _F] + _TAIL,
     'effdet_nms_batch': [_P, _P, _P, _INT, _INT, _INT, _INT, ctypes.c_double, _P, _P, _P] + _TAIL,
+    'effdet_nms_batch_chunked': [_P, _P, _P] + [_INT] * 5 + [ctypes.c_double, _P, _I64, _P, _P] + _TAIL,
     'effdet_gather_detections_batch': [_P, _P, _P, _P, _P, _INT, _INT, _INT, _P, _P, _P] + _TAIL,
     'effdet_multi_sumsq': [_P, _P, _P, _P, _INT, _INT, _P] + _TAIL,
     'effdet_multi_clip_adamw': [_P] * 7 + [_INT, _INT, _P] + [_F] * 8 + [_INT] + _TAIL,
@@ -179,7 +180,8 @@ PLAIN = {'effdet_version': (ctypes.c_int, []), 'effdet_conv_tc_kpad': (ctypes.c_
          'effdet_wgrad_tc_geometry_ok': (ctypes.c_int, [ctypes.c_int] * 3), 'effdet_last_error': (ctypes.c_char_p, []),
          'effdet_launch_count': (ctypes.c_uint64, []), 'effdet_reset_launch_count': (None, []),
          'effdet_voc_ap_workspace': (ctypes.c_int64, [ctypes.c_int] * 2),
-         'effdet_coco_accumulate_workspace': (ctypes.c_int64, [ctypes.c_int] * 3)}
+         'effdet_coco_accumulate_workspace': (ctypes.c_int64, [ctypes.c_int] * 3),
+         'effdet_nms_chunked_workspace': (ctypes.c_int64, [ctypes.c_int] * 3)}
 
 _lib = None
 _lock = threading.Lock()

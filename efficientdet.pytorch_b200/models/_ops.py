@@ -1009,11 +1009,33 @@ class FocalLossFn(torch.autograd.Function):
 # ------------------------------------------------------------------------------------------------
 
 
-# Bytes the eager NMS mask workspace may take before the batch is split into consecutive groups of images (at least one
-# image per group).  Realistic candidate counts keep the whole batch in one group: 5 k candidates cost 3.2 MB per image.
+# Bytes the NMS workspace may take before the batch is split into consecutive groups of images (at least one image per
+# group).  Realistic candidate counts keep the whole batch in one group: 5 k candidates cost 3.2 MB per image.
 NMS_MASK_BUDGET = 1 << 30
 
+# Column chunk of the NMS for cap > NMS_CHUNK (effdet_nms_batch_chunked): the workspace is NMS_CHUNK * NMS_CHUNK / 8
+# bytes of mask per image (2 MiB at 4096), whatever the candidate count.  Up to NMS_CHUNK candidates NMS runs as one
+# chunk, which is the square-mask path.  4096 keeps every realistic candidate count (a few thousand) on that path
+# unchanged.  Measured (tools/bench_detect.py chunk_sweep; H100 80GB HBM3, 700 W), chunk 1024 / 2048 / 4096 / 8192:
+# D0 512^2 bs 32 with all 49 104 anchors 16.4 / 16.4 / 17.9 / 22.3 ms, the D7 bench image (327 867 candidates)
+# 52.5 / 49.7 / 49.5 / 49.3 ms.
+NMS_CHUNK = 4096
+
 Detections = collections.namedtuple('Detections', 'scores classes boxes count')
+
+
+def candidate_cap(max_candidates, cls):
+    """the fixed cap detect_batch gets for cls [B,A,K]: max_candidates clamped to A, or A for None"""
+    A = cls.shape[1]
+    return A if max_candidates is None else min(int(max_candidates), A)
+
+
+def _nms_workspace(B, cap, chunk):
+    """bytes of effdet_nms_batch_chunked's workspace"""
+    n = int(N.load().effdet_nms_chunked_workspace(B, cap, chunk))
+    if n < 0:
+        raise N.EffdetNativeError('detect_batch: %s' % N.last_error())
+    return n
 
 
 def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=None):
@@ -1047,15 +1069,17 @@ def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=
         if cap == 0:
             return [[cls.new_zeros(0), torch.zeros(0, dtype=torch.int64, device=dev), cls.new_zeros(0, 4)]
                     for _ in range(B)]
-    cw = (cap + 63) // 64
-    per_image = cap * cw * 8
+    chunk = min(cap, NMS_CHUNK)
+    per_image = _nms_workspace(1, cap, chunk)
     group = min(B, max(NMS_MASK_BUDGET, per_image) // per_image)
-    mask = torch.empty((group * cap * cw,), device=dev, dtype=torch.int64)
+    ws_bytes = _nms_workspace(group, cap, chunk)
+    ws = torch.empty((ws_bytes // 8,), device=dev, dtype=torch.int64)
     keep = torch.empty((B, cap), device=dev, dtype=torch.int32)
     nkeep = torch.empty((B,), device=dev, dtype=torch.int32)
     for b0 in range(0, B, group):
-        N.call('effdet_nms_batch', cls, N.f32(boxes[b0:]), keys[b0:].data_ptr(), count[b0:].data_ptr(), min(group, B - b0),
-               A, npad, cap, float(iou_threshold), mask.data_ptr(), keep[b0:].data_ptr(), nkeep[b0:].data_ptr())
+        N.call('effdet_nms_batch_chunked', cls, N.f32(boxes[b0:]), keys[b0:].data_ptr(), count[b0:].data_ptr(),
+               min(group, B - b0), A, npad, cap, chunk, float(iou_threshold), ws.data_ptr(), ws_bytes,
+               keep[b0:].data_ptr(), nkeep[b0:].data_ptr())
     o_s = _empty((B, cap), cls)
     o_c = torch.empty((B, cap), device=dev, dtype=torch.int64)
     o_b = _empty((B, cap, 4), cls)

@@ -23,8 +23,9 @@ from . import _native as N
 from . import _ops
 from .graph_step import GraphedDetect
 
-# candidate rows per image that the graphed detection keeps before NMS; an image with more is redone eagerly
-MAX_CANDIDATES = 8192
+# candidate rows per image that the graphed detection keeps before NMS: None = every anchor, so no image overflows; with
+# an integer, an image with more candidates is redone eagerly
+MAX_CANDIDATES = None
 
 
 class VOCAccumulator:
@@ -156,7 +157,7 @@ def _detect_all(dataset, model, acc, batch_size, per_image, progress_base):
             else:
                 cls, reg, anchors = model._raw_predictions(images)
                 out = _ops.detect_batch(cls, reg, anchors, hw[0], hw[1], model.threshold, model.iou_threshold,
-                                        cap=min(MAX_CANDIDATES, cls.shape[1]))
+                                        cap=_ops.candidate_cap(MAX_CANDIDATES, cls))
             _add_batch(acc, out, cls, reg, anchors, hw, model, [d['scale'] for d in data], *per_image(idx))
             for i in idx:
                 print('{}/{}'.format(i + progress_base, n), end='\r')

@@ -159,12 +159,14 @@ class GraphedDetect:
 
     out.scores [B,C], out.classes [B,C] int64, out.boxes [B,C,4] and out.count [B] int32 (kept rows; -1 when the image
     has more than C candidates above the threshold) are static tensors: every call rewrites them.  C is max_candidates,
-    or the anchor count A when that is smaller (an image never has more than A candidates).  to_list redoes overflowed
-    images eagerly from the network outputs of the last replay.  Calls take images of the example's shape only.
+    or the anchor count A when that is smaller (an image never has more than A candidates); max_candidates=None sets
+    C = A, so every anchor may be a candidate and no image overflows.  to_list redoes overflowed images eagerly from the
+    network outputs of the last replay.  Calls take images of the example's shape only.
 
-    Memory that max_candidates costs per image: the NMS mask C * ceil(C/64) * 8 bytes (8 MiB at C = 8192) plus
-    32 bytes per row of keep indices and padded outputs.  The decoded anchors and their sort keys (24 bytes per anchor
-    plus 8 per power-of-two padded anchor) do not depend on C.
+    Memory that max_candidates costs per image is linear in C: 32 bytes per row of keep indices and padded outputs,
+    plus the NMS workspace, which is the mask C * ceil(C/64) * 8 bytes up to C = _ops.NMS_CHUNK and the mask of one
+    chunk (2 MiB at NMS_CHUNK = 4096) above it.  At D7 1536x1536 (A = 441 936) C = A costs about 16 MB per image.  The
+    decoded anchors and their sort keys (24 bytes per anchor plus 8 per power-of-two padded anchor) do not depend on C.
 
     The packed weights and folded BatchNorm are derived inside the graph, so replays follow in-place weight updates
     (load_state_dict, EMA copies).  The score and IoU thresholds are fixed at capture."""
@@ -176,7 +178,7 @@ class GraphedDetect:
         if not images.is_cuda:
             raise _ops.N.EffdetNativeError('GraphedDetect needs CUDA example images')
         self.model = model
-        self.max_candidates = int(max_candidates)
+        self.max_candidates = None if max_candidates is None else int(max_candidates)
         self.threshold, self.iou_threshold = model.threshold, model.iou_threshold
         self.static_images = images.clone()
         dev = images.device
@@ -201,7 +203,7 @@ class GraphedDetect:
     def _run(self):
         cls, reg, anchors = self.model._raw_predictions(self.static_images)
         out = _ops.detect_batch(cls, reg, anchors, self.static_images.shape[2], self.static_images.shape[3],
-                                self.threshold, self.iou_threshold, cap=min(self.max_candidates, cls.shape[1]))
+                                self.threshold, self.iou_threshold, cap=_ops.candidate_cap(self.max_candidates, cls))
         return cls, reg, anchors, out
 
     def __call__(self, images):

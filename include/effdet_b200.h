@@ -340,6 +340,18 @@ int effdet_detect_candidates_batch(const float* cls, const float* reg, const flo
 int effdet_nms_batch(const float* boxes, const uint64_t* keys, const int32_t* count, int B, int A, int npad, int cap,
                      double iou_threshold, uint64_t* mask_ws, int32_t* keep_idx, int32_t* nkeep, int device,
                      effdet_stream_t stream);
+/* The same greedy NMS in column chunks of `chunk` sorted candidates, in a workspace linear in cap: for each chunk, a
+ * cross step tests its candidates against the boxes kept so far (through keep_idx), then the upper-triangle mask and
+ * the greedy scan run inside the chunk.  The keep sets, their order and nkeep equal effdet_nms_batch's for every chunk;
+ * chunk == cap is effdet_nms_batch itself.  The launch sequence depends on B, cap and chunk only (capturable).
+ *   1 <= B <= 65535; 1 <= cap <= A (any cap: only the chunk's bitmap lives in shared memory);
+ *   chunk a multiple of 64 in [64, cap], or chunk == cap
+ *   workspace: effdet_nms_chunked_workspace(B, cap, chunk) bytes, 16-byte aligned (-1 when the arguments are refused)
+ *   keep_idx, nkeep: as effdet_nms_batch */
+int64_t effdet_nms_chunked_workspace(int B, int cap, int chunk);
+int effdet_nms_batch_chunked(const float* boxes, const uint64_t* keys, const int32_t* count, int B, int A, int npad,
+                             int cap, int chunk, double iou_threshold, void* workspace, int64_t workspace_bytes,
+                             int32_t* keep_idx, int32_t* nkeep, int device, effdet_stream_t stream);
 /* Padded detections: row i < nkeep[b] of image b is its i-th kept box, every later row is zero (all rows when
  * nkeep[b] == -1).  out_scores [B][cap] float, out_classes [B][cap] int64, out_boxes [B][cap][4] float (16-byte aligned). */
 int effdet_gather_detections_batch(const float* boxes, const float* scores, const int32_t* classes,

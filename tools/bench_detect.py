@@ -13,8 +13,11 @@ One measurement per process, in the source tree given by --tree (default: this o
                           and the device time of each post-processing kernel (torch.profiler, after the timed loops).
 
 The driver alternates this tree and the tree given by --parent (a checkout of an earlier commit whose library has been
-built), RUNS processes each for `post` and `d7_split` and RUNS runs of `bench.py --config d7 --dump-outputs` each, and reads the card's name, power limit and maximum SM clock in the same call:
-  python tools/bench_detect.py --driver 5 --parent DIR --out DIR [--legs eager_vs_graph,post,d7_split,bench]
+built), RUNS processes each for `post` and `d7_split` and RUNS runs of `bench.py --config d7 --dump-outputs` each, and reads the card's name, power limit and maximum SM clock in the same call.  The `chunk_sweep` leg runs this tree
+once after the alternated runs: post-processing time, peak memory and output hash per _ops.NMS_CHUNK, on D0 bs 32 with
+every anchor a candidate and on the D7 bench image.  `post` and `d7_split` also report the peak memory the
+post-processing allocates.
+  python tools/bench_detect.py --driver 5 --parent DIR --out DIR [--legs eager_vs_graph,post,d7_split,chunk_sweep,bench]
 """
 import argparse
 import hashlib
@@ -52,6 +55,16 @@ def _post(_ops, cls, reg, anchors, h, w, thr):
     if hasattr(_ops, 'detect_batch'):
         return _ops.detect_batch(cls, reg, anchors, h, w, thr, 0.5)
     return [_ops.detect_image0(cls, reg, anchors, h, w, thr, 0.5, index=i) for i in range(cls.shape[0])]
+
+
+def _peak_mb(torch, fn):
+    """device memory fn allocates at its peak beyond what was allocated before it, MB"""
+    torch.cuda.synchronize()
+    base = torch.cuda.memory_allocated()
+    torch.cuda.reset_peak_memory_stats()
+    fn()
+    torch.cuda.synchronize()
+    return round((torch.cuda.max_memory_allocated() - base) / 1e6, 1)
 
 
 def _wall(torch, fn, n):
@@ -120,6 +133,7 @@ def part_post(tree, iters):
                 h.update(t.detach().cpu().numpy().tobytes())
         res[name] = dict(threshold=thr, candidates_min_max=n, kept_total=sum(int(t[0].numel()) for t in out if t),
                          ms=_wall(torch, lambda: _post(_ops, cls, reg, anchors, S, S, thr), iters if thr > 0 else 2),
+                         peak_mb=_peak_mb(torch, lambda: _post(_ops, cls, reg, anchors, S, S, thr)),
                          sha256=h.hexdigest()[:16])
     return res
 
@@ -143,6 +157,7 @@ def part_d7_split(tree, iters, io):
         res['candidates'] = int((cls.max(dim=2)[0] > 0.4).sum())
         res['network_ms'] = _wall(torch, lambda: model._raw_predictions(x), iters)
         res['post_ms'] = _wall(torch, lambda: _post(_ops, cls[:1], reg[:1], anchors, 1536, 1536, 0.4), iters)
+        res['post_peak_mb'] = _peak_mb(torch, lambda: _post(_ops, cls[:1], reg[:1], anchors, 1536, 1536, 0.4))
         res['forward_ms'] = _wall(torch, lambda: model(x), iters)
         h = hashlib.sha256()
         for t in _post(_ops, cls[:1], reg[:1], anchors, 1536, 1536, 0.4)[0]:
@@ -158,6 +173,35 @@ def part_d7_split(tree, iters, io):
             if str(e.device_type).endswith('CUDA'):
                 k[e.name[:40]] = k.get(e.name[:40], 0.0) + getattr(e, 'device_time_total', 0.0) / 1e3
         res['post_kernel_ms'] = {n: round(v, 3) for n, v in sorted(k.items(), key=lambda kv: -kv[1])[:8]}
+    return res
+
+
+def part_chunk_sweep(tree, iters, io):
+    """this tree only: post-processing ms and peak MB per NMS_CHUNK, on D0 512x512 bs 32 with every anchor a candidate
+    and on the D7 bench image's network outputs (--io, written by d7_split); the hashes must not depend on the chunk"""
+    torch, _, _ops, O, _ = _import(tree)
+    dev = torch.device('cuda', 0)
+    res = dict(part='chunk_sweep')
+    B, K, S = 32, 80, 512
+    a0 = torch.from_numpy(O.anchors_for(S, S)).to(dev)
+    g = torch.Generator().manual_seed(7)
+    cls0 = torch.rand(B, a0.shape[1], K, generator=g).to(dev)
+    reg0 = (torch.randn(B, a0.shape[1], 4, generator=g) * 0.3).to(dev)
+    cases = [('d0 bs32 all anchors', cls0, reg0, a0, S, -1.0, 2)]
+    if io and os.path.exists(io):
+        cls7, reg7 = [t.to(dev) for t in torch.load(io)]
+        cases.append(('d7 bench image', cls7[:1], reg7[:1], torch.from_numpy(O.anchors_for(1536, 1536)).to(dev), 1536,
+                      0.4, iters))
+    for chunk in (1024, 2048, 4096, 8192):
+        _ops.NMS_CHUNK = chunk
+        for name, cls, reg, anchors, s, thr, n in cases:
+            run = lambda: _post(_ops, cls, reg, anchors, s, s, thr)  # noqa: E731
+            h = hashlib.sha256()
+            for trip in run():
+                for t in trip:
+                    h.update(t.cpu().numpy().tobytes())
+            res['%s chunk %d' % (name, chunk)] = dict(ms=_wall(torch, run, n), peak_mb=_peak_mb(torch, run),
+                                                     sha256=h.hexdigest()[:16])
     return res
 
 
@@ -197,18 +241,22 @@ def driver(runs, parent, out, iters, legs):
         if 'post' in legs:
             for case in ('realistic', 'all_anchors'):
                 s['post bs32 %s ms' % case] = med([r['post'][case]['ms'] for r in rs])
+                s['post bs32 %s peak MB' % case] = rs[-1]['post'][case].get('peak_mb')
                 s['post bs32 %s sha256' % case] = sorted({r['post'][case]['sha256'] for r in rs})
                 s['post bs32 %s candidates min/max' % case] = rs[0]['post'][case]['candidates_min_max']
         if 'd7_split' in legs:
             for f in ('network_ms', 'post_ms', 'forward_ms'):
                 s['d7 ' + f] = med([r['d7_split'][f] for r in rs])
             s['d7 candidates'] = rs[0]['d7_split']['candidates']
+            s['d7 post peak MB'] = rs[-1]['d7_split'].get('post_peak_mb')
             s['d7 post sha256'] = sorted({r['d7_split']['sha256'] for r in rs})
             s['d7 post kernel ms (last run)'] = rs[-1]['d7_split']['post_kernel_ms']
         if 'bench' in legs:
             s['bench d7 img/s'] = med([r['bench']['value'] for r in rs])
         if s:
             summary[k] = s
+    if 'chunk_sweep' in legs:
+        summary['chunk_sweep'] = _run([sys.executable, me, '--part', 'chunk_sweep', '--iters', str(iters), '--io', io])
     if 'bench' in legs:
         # detections of separate processes differ by the network's fp32 atomics; the post-processing alone is compared
         # bit for bit by the d7_split leg
@@ -224,7 +272,7 @@ def driver(runs, parent, out, iters, legs):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--part', choices=['eager_vs_graph', 'post', 'd7_split'])
+    ap.add_argument('--part', choices=['eager_vs_graph', 'post', 'd7_split', 'chunk_sweep'])
     ap.add_argument('--tree', default=R, help='source tree whose library to measure')
     ap.add_argument('--iters', type=int, default=20)
     ap.add_argument('--driver', type=int, default=0, metavar='RUNS', help='alternate parent and this tree RUNS times')
@@ -237,8 +285,8 @@ def main():
         os.makedirs(args.out, exist_ok=True)
         driver(args.driver, args.parent, args.out, args.iters, args.legs.split(','))
     else:
-        if args.part == 'd7_split':
-            res = part_d7_split(args.tree, args.iters, args.io)
+        if args.part in ('d7_split', 'chunk_sweep'):
+            res = dict(d7_split=part_d7_split, chunk_sweep=part_chunk_sweep)[args.part](args.tree, args.iters, args.io)
         else:
             res = dict(eager_vs_graph=part_eager_vs_graph, post=part_post)[args.part](args.tree, args.iters)
         print(json.dumps(res), flush=True)

@@ -1,5 +1,6 @@
 """VOC evaluation timing on one GPU: the device accumulator (models/evaluation.py) against the host accumulation, and
-evaluate() end to end against the reference-style loop (one image per forward, host selection and accumulation).
+evaluate() end to end against the reference-style loop (one image per forward, host selection and accumulation), at
+the default MAX_CANDIDATES and at 8192.
 
 usage: python tools/bench_eval.py [--images 4952] [--e2e-images 256] [--batch 16]
 Prints one JSON line with the card name and power limit read in the same run."""
@@ -122,13 +123,25 @@ def end_to_end(n, batch, size=512, K=20):
         t = time.perf_counter()
         got = evaluation.evaluate(gen, m, batch_size=batch)
         dev_s = time.perf_counter() - t
+        default = evaluation.MAX_CANDIDATES
+        evaluation.MAX_CANDIDATES = 8192                              # the cap before every anchor could be a candidate
+        try:
+            evaluation.evaluate(warm, m, batch_size=batch)
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            got_8192 = evaluation.evaluate(gen, m, batch_size=batch)
+            dev_8192_s = time.perf_counter() - t
+        finally:
+            evaluation.MAX_CANDIDATES = default
         t = time.perf_counter()
         ref = V.evaluate(V.get_detections(gen, m), V.get_annotations(gen), K)
         ref_s = time.perf_counter() - t
     finally:
         sys.stdout = out
-    return dict(images=n, size=size, batch=batch, evaluate_img_s=round(n / dev_s, 1), reference_loop_img_s=round(n / ref_s, 1),
-                mean_ap_device=float(got[0]), mean_ap_reference_loop=float(ref[0]))
+    return dict(images=n, size=size, batch=batch, max_candidates=repr(default), evaluate_img_s=round(n / dev_s, 1),
+                evaluate_max_candidates_8192_img_s=round(n / dev_8192_s, 1), reference_loop_img_s=round(n / ref_s, 1),
+                mean_ap_device=float(got[0]), mean_ap_max_candidates_8192=float(got_8192[0]),
+                mean_ap_reference_loop=float(ref[0]))
 
 
 def main():
