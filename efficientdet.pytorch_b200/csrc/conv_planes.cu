@@ -18,11 +18,16 @@
 //               accumulator in registers (single-pass instance, NP = 1: hi*hi only, and the producer loads no lo plane),
 //               then the epilogue: bias / ReLU / sigmoid / ReLU-mask / residual -> bf16 hi/lo planes (the next layer's
 //               operand) and / or fp32 (head outputs, data gradient w.r.t. the BiFPN features); optional per-channel
-//               column sums of what was stored (= the bias gradient of the producing layer) reduced by warp shuffles,
-//               one atomic per column per warp.  One warpgroup's epilogue runs under the other's MMAs.
+//               column sums of what was stored (= the bias gradient of the producing layer) reduced by warp shuffles
+//               into the CTA's [Cout] array (shared atomics), added to colsum once per CTA.  One warpgroup's epilogue
+//               runs under the other's MMAs.
 // persistent over (pixel tile, channel tile) units of all pyramid levels that share the weights.
+// A ReLU forward can also write the one-bit mask its data gradient applies (y_mask: bit c % 32 of word (pixel, c / 32)
+// <=> the stored value of channel c is > 0); a data gradient given mask_bits loads its words before its last MMAs
+// complete, 4 bytes per 32 channels instead of 2 x 64 bytes of planes read after them.
 #include "tc_ptx.cuh"
 
+#include <limits.h>
 #include <stdlib.h>
 
 namespace effdet {
@@ -33,8 +38,10 @@ constexpr int kPlMaxLevels = 8;
 constexpr int kPlThreads = 384;
 constexpr int kPlProducerRegs = 40, kPlConsumerRegs = 232;
 constexpr int kPlA = 128 * 128;            // one plane of the activation tile: 128 pixel rows x 64 channels (bf16)
+constexpr int kPlSmemOptin = 227 * 1024;   // sm_90's dynamic shared memory per block
 // BN = output channels per tile (accumulator: BN registers per consumer thread); the ring depth is what fits.  Behind
-// the ring: the two warpgroups' staging buffers (wg_rows_own), the mbarriers, the two warpgroups' bias buffers.
+// the ring: the two warpgroups' staging buffers (wg_rows_own), the mbarriers, the two warpgroups' bias buffers, and in
+// a launch with column sums the CTA's [Cout] array of them (not counted in kSmem).
 template <int BN>
 struct PlCfg {
     static constexpr int kStages = BN == 128 ? 3 : 4;
@@ -42,8 +49,23 @@ struct PlCfg {
     static constexpr int kStage = 2 * kPlA + 2 * kB;
     static constexpr int kSmem = kStages * kStage + kRowsBytes + 1024 + 256 + 2 * BN * 4;
 };
-// named barriers of the consumer warpgroup g: 2 + g its staging buffer and bias buffer, 4 + g its turn to consume
-constexpr int kPlBarRows = 2, kPlBarTurn = 4;
+// named barriers: 1 both consumer warpgroups (their column sums are complete), 2 + g the staging buffer and bias
+// buffer of consumer warpgroup g, 4 + g its turn to consume
+constexpr int kPlBarSums = 1, kPlBarRows = 2, kPlBarTurn = 4;
+
+// bit e (0..7) set <=> the value stored as the bf16 pair (hi, lo) of channel e is > 0: sign clear and magnitude
+// bits set, in hi or, where hi is zero, in lo
+__device__ __forceinline__ uint32_t relu_bits8(const uint4 hi, const uint4 lo) {
+    const uint32_t hw[4] = {hi.x, hi.y, hi.z, hi.w}, lw[4] = {lo.x, lo.y, lo.z, lo.w};
+    uint32_t bits = 0;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        const uint32_t hb = (hw[e >> 1] >> ((e & 1) * 16)) & 0xffffu, lb = (lw[e >> 1] >> ((e & 1) * 16)) & 0xffffu;
+        const bool pos = (hb & 0x7fffu) ? !(hb & 0x8000u) : ((lb & 0x7fffu) && !(lb & 0x8000u));
+        bits |= (uint32_t)pos << e;
+    }
+    return bits;
+}
 
 struct PlLevel {
     int B, H, W;
@@ -54,19 +76,35 @@ struct PlLevel {
     long long y_bstride;
     __nv_bfloat16* y_planes;               // bf16 hi/lo output planes [2][B*H*W][opitch], or NULL
     const __nv_bfloat16* mask_planes;      // ReLU-backward mask source [2][B*H*W][opitch] (value > 0 keeps the gradient), or NULL
+    uint32_t* y_mask;                      // ReLU bits of the stored planes [B*H*W][mwords], or NULL
+    const uint32_t* mask_bits;             // ReLU-backward mask as bits [B*H*W][mwords] (set keeps the gradient), or NULL
     const float* residual;                 // fp32 [B][H*W][Cout] added last, or NULL
     long long r_bstride;
 };
 struct PlArgs {
     PlLevel lv[kPlMaxLevels];
     int nlevels, total_tiles, ntn;
-    int Cin, Cout, ksize, act, kblocks, opitch;
+    int Cin, Cout, ksize, act, kblocks, opitch, mwords;
     const float* bias;                     // [Cout] or NULL
     float* colsum;                         // [Cout] += column sums of the stored values, or NULL
 };
 struct PlMaps {
     CUtensorMap x[kPlMaxLevels];
 };
+
+// one step of a warp transpose-reduce of v[0 .. 2 OFF - 1]: lanes with bit OFF set keep the upper half, the others the
+// lower one, and each adds its partner's copy of the half it keeps.  A compile-time OFF keeps v in registers (a loop
+// over OFF that is not unrolled indexes v at run time, which puts it in local memory).
+template <int OFF>
+__device__ __forceinline__ void transpose_add(float (&v)[32], const int lane) {
+    const bool upper = (lane & OFF) != 0;
+#pragma unroll
+    for (int k = 0; k < OFF; ++k) {
+        const float send = upper ? v[k] : v[k + OFF];
+        const float keep = upper ? v[k + OFF] : v[k];
+        v[k] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
+    }
+}
 
 // NP = bf16 products per multiply-add: 3 (split precision) or 1 (hi planes only)
 template <int BN, int NP>
@@ -79,6 +117,7 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kPlStages * kPlStage + kRowsBytes);
     uint64_t* empty_bar = full_bar + kPlStages;
     float* chan_buf = reinterpret_cast<float*>(smem + kPlStages * kPlStage + kRowsBytes + 256);   // bias of the channel tile
+    float* csum = chan_buf + 2 * kPlBN;                                             // the CTA's column sums [Cout]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int taps = P.ksize * P.ksize, pad = P.ksize / 2;
@@ -91,6 +130,8 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
         fence_barrier_init();
         tma_prefetch_desc(&wmap);
     }
+    if (P.colsum)
+        for (int i = threadIdx.x; i < P.Cout; i += kPlThreads) csum[i] = 0.f;
     __syncthreads();
 
     // unit -> (level, first box of the pixel tile, first output channel)
@@ -179,6 +220,36 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                 if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kPlStages]);
             }
             if (k + 1 < nunits) named_bar_arrive(kPlBarTurn + (g ^ 1), 256);
+            const int ncols = min(kPlBN, P.Cout - n0);
+            const int nchunks = (ncols + 31) >> 5;
+            // under the last MMAs: the pixel of the row this thread finishes in each row half (-1 past the map), and
+            // the mask words of its chunks
+            int pix[2];                                            // < 2^31: B * H * W is checked on the host
+            uint32_t mbits[2][NB];
+#pragma unroll
+            for (int m = 0; m < 2; ++m) {
+                // pixel of row r: box q of the tile, position i inside the box (x fastest, then y, then image)
+                const int r = m * 64 + (warp & 1) * 32 + lane;
+                const int ks = L.g.kstage;
+                const int q = r / ks, i = r - q * ks;
+                int ch = box0 + q;
+                const bool box_ok = ch < L.nboxes;
+                const int bx = ch % L.g.nbx;
+                ch /= L.g.nbx;
+                const int by = ch % L.g.nby;
+                const int bb = ch / L.g.nby;
+                const int wh = L.g.Wb * L.g.Hb;
+                const int bi = i / wh, rem = i - bi * wh;
+                const int yy = rem / L.g.Wb, xx = rem - yy * L.g.Wb;
+                const int b = bb * L.g.Bb + bi, y = by * L.g.Hb + yy, x = bx * L.g.Wb + xx;
+                pix[m] = box_ok && b < L.B ? (b * L.H + y) * L.W + x : -1;
+#pragma unroll
+                for (int jb = 0; jb < NB; ++jb) {
+                    const int cc = 2 * jb + half;
+                    mbits[m][jb] = L.mask_bits && pix[m] >= 0 && cc < nchunks
+                                       ? __ldg(L.mask_bits + (long long)pix[m] * P.mwords + (n0 >> 5) + cc) : 0u;
+                }
+            }
             wgmma_wait<0>();
             if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kPlStages]);
             if (n0 != chan_n0) {
@@ -188,31 +259,23 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                 chan_n0 = n0;
             }
             const long long plane = (long long)L.B * L.H * L.W * P.opitch;
-            const int ncols = min(kPlBN, P.Cout - n0);
-            const int nchunks = (ncols + 31) >> 5;
+            // One copy of the block epilogue, looped over the 2 x NB blocks (only the staging, which must name its
+            // accumulator block statically, is unrolled): unrolled per block, the kernel's code grew past what the
+            // SMs' instruction caches hold, and every launch paid for it, with or without mask, residual or sums.
+#pragma unroll 1
+            for (int blk = 0; blk < 2 * NB; ++blk) {
+                const int m = blk / NB, jb = blk - m * NB;
+                float v[32];
+                uint32_t keep_bits = 0;
 #pragma unroll
-            for (int m = 0; m < 2; ++m) {
-                // pixel of row r: box q of the tile, position i inside the box (x fastest, then y, then image)
-                const int r = m * 64 + (warp & 1) * 32 + lane;         // row of the tile owned by this thread
-                const int ks = L.g.kstage;
-                const int q = r / ks, i = r - q * ks;
-                int ch = box0 + q;
-                bool row_ok = ch < L.nboxes;
-                const int bx = ch % L.g.nbx;
-                ch /= L.g.nbx;
-                const int by = ch % L.g.nby;
-                const int bb = ch / L.g.nby;
-                const int wh = L.g.Wb * L.g.Hb;
-                const int bi = i / wh, rem = i - bi * wh;
-                const int yy = rem / L.g.Wb, xx = rem - yy * L.g.Wb;
-                const int b = bb * L.g.Bb + bi, y = by * L.g.Hb + yy, x = bx * L.g.Wb + xx;
-                row_ok = row_ok && b < L.B;
-                const long long pixb = (long long)y * L.W + x;                     // pixel inside its image
-                const long long pix = (long long)b * L.H * L.W + pixb;             // pixel in the planes
-#pragma unroll
-                for (int jb = 0; jb < NB; ++jb) {
-                    float v[32];
-                    wg_rows_own(d[m][jb], rows, kPlBarRows + g, v);
+                for (int q = 0; q < 2 * NB; ++q)
+                    if (q == blk) {
+                        wg_rows_own(d[q / NB][q % NB], rows, kPlBarRows + g, v);
+                        keep_bits = mbits[q / NB][q % NB];
+                    }
+                {
+                    const int pix_ = m ? pix[1] : pix[0];                      // pixel in the planes of the row
+                    const bool row_ok = pix_ >= 0;                             // ... this thread owns
                     const int cc = 2 * jb + half;
                     if (cc >= nchunks) continue;
                     const int nb = n0 + cc * 32;                        // first channel of the chunk
@@ -224,28 +287,30 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                         v[k] = t;
                     }
                     if (row_ok && L.residual) {
+                        const int hw = L.H * L.W, b = pix_ / hw, pixb = pix_ - b * hw;        // image, pixel inside it
 #pragma unroll
                         for (int k4 = 0; k4 < 8; ++k4) {
                             if (nb + k4 * 4 >= P.Cout) break;
-                            const float4 rv = ldg4(L.residual + (long long)b * L.r_bstride + pixb * P.Cout + nb + k4 * 4);
+                            const float4 rv = ldg4(L.residual + (long long)b * L.r_bstride + (long long)pixb * P.Cout + nb + k4 * 4);
                             v[k4 * 4] += rv.x; v[k4 * 4 + 1] += rv.y; v[k4 * 4 + 2] += rv.z; v[k4 * 4 + 3] += rv.w;
                         }
                     }
-                    if (row_ok && L.mask_planes) {                     // gradient passes where the forward activation was > 0
-                        const __nv_bfloat16* mh = L.mask_planes + pix * P.opitch + nb;
+                    // gradient passes where the forward activation was > 0
+                    if (L.mask_bits) {
+                        const uint32_t keep = keep_bits;
+#pragma unroll
+                        for (int k = 0; k < 32; ++k)
+                            if (!((keep >> k) & 1u)) v[k] = 0.f;
+                    } else if (row_ok && L.mask_planes) {
+                        const __nv_bfloat16* mh = L.mask_planes + (long long)pix_ * P.opitch + nb;
 #pragma unroll
                         for (int k8 = 0; k8 < 4; ++k8) {
                             if (nb + k8 * 8 >= P.Cout) break;
-                            const uint4 hv = __ldg(reinterpret_cast<const uint4*>(mh + k8 * 8));
-                            const uint4 lv = __ldg(reinterpret_cast<const uint4*>(mh + plane + k8 * 8));
-                            const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
+                            const uint32_t keep = relu_bits8(__ldg(reinterpret_cast<const uint4*>(mh + k8 * 8)),
+                                                             __ldg(reinterpret_cast<const uint4*>(mh + plane + k8 * 8)));
 #pragma unroll
-                            for (int e = 0; e < 8; ++e) {
-                                const uint32_t hb = (hw[e >> 1] >> ((e & 1) * 16)) & 0xffffu, lb = (lw[e >> 1] >> ((e & 1) * 16)) & 0xffffu;
-                                // bf16 bits: positive and non-zero  <=>  sign clear and magnitude bits set
-                                const bool pos = (hb & 0x7fffu) ? !(hb & 0x8000u) : ((lb & 0x7fffu) && !(lb & 0x8000u));
-                                if (!pos) v[k8 * 8 + e] = 0.f;
-                            }
+                            for (int e = 0; e < 8; ++e)
+                                if (!((keep >> e) & 1u)) v[k8 * 8 + e] = 0.f;
                         }
                     }
                     if (!row_ok) {
@@ -253,7 +318,8 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                         for (int k = 0; k < 32; ++k) v[k] = 0.f;
                     }
                     if (row_ok && L.y) {
-                        float* yo = L.y + (long long)b * L.y_bstride + pixb * P.Cout + nb;
+                        const int hw = L.H * L.W, b = pix_ / hw, pixb = pix_ - b * hw;
+                        float* yo = L.y + (long long)b * L.y_bstride + (long long)pixb * P.Cout + nb;
 #pragma unroll
                         for (int k4 = 0; k4 < 8; ++k4) {
                             if (nb + k4 * 4 >= P.Cout) break;
@@ -261,7 +327,8 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                         }
                     }
                     if (row_ok && L.y_planes) {
-                        __nv_bfloat16* ph = L.y_planes + pix * P.opitch + nb;
+                        __nv_bfloat16* ph = L.y_planes + (long long)pix_ * P.opitch + nb;
+                        uint32_t word = 0;                             // y_mask of the chunk: channel nb + k is bit k
 #pragma unroll
                         for (int k8 = 0; k8 < 4; ++k8) {
                             if (nb + k8 * 8 >= P.Cout) break;
@@ -270,24 +337,25 @@ conv_planes_kernel(const __grid_constant__ PlMaps maps, const __grid_constant__ 
                                    make_float4(v[k8 * 8 + 4], v[k8 * 8 + 5], v[k8 * 8 + 6], v[k8 * 8 + 7]), hi, lo);
                             *reinterpret_cast<uint4*>(ph + k8 * 8) = hi;
                             *reinterpret_cast<uint4*>(ph + plane + k8 * 8) = lo;
+                            if (L.y_mask) word |= relu_bits8(hi, lo) << (8 * k8);
                         }
+                        if (L.y_mask) L.y_mask[(long long)pix_ * P.mwords + (nb >> 5)] = word;
                     }
                     if (P.colsum) {
                         // warp transpose-reduce: afterwards v[0] of lane j is the sum over the warp's 32 rows of column j
-#pragma unroll
-                        for (int off = 16; off >= 1; off >>= 1) {
-                            const bool upper = (lane & off) != 0;
-#pragma unroll
-                            for (int k = 0; k < off; ++k) {
-                                const float send = upper ? v[k] : v[k + off];
-                                const float keep = upper ? v[k + off] : v[k];
-                                v[k] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                            }
-                        }
-                        if (nb + lane < P.Cout) atomicAdd(P.colsum + nb + lane, v[0]);
+                        transpose_add<16>(v, lane);
+                        transpose_add<8>(v, lane);
+                        transpose_add<4>(v, lane);
+                        transpose_add<2>(v, lane);
+                        transpose_add<1>(v, lane);
+                        if (nb + lane < P.Cout) atomicAdd(csum + nb + lane, v[0]);
                     }
                 }
             }
+        }
+        if (P.colsum) {
+            named_bar_sync(kPlBarSums, 256);                           // both warpgroups' sums are in csum
+            for (int i = threadIdx.x; i < P.Cout; i += 256) atomicAdd(P.colsum + i, csum[i]);
         }
     }
 }
@@ -400,6 +468,16 @@ extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, i
     EFFDET_REQUIRE(a0->w_tc && (a0->ksize == 1 || a0->ksize == 3) && a0->Cin % 4 == 0 && a0->Cout % 4 == 0 && a0->Cin >= 8 &&
                        a0->Cout >= 8,
                    "conv_planes_multi: needs the bf16 weight pack, k in {1,3}, channels %% 4 == 0");
+    // 128 x 128 tiles at most: the accumulator lives in the consumer warpgroups' registers (64 per thread)
+    const int BN = a0->Cout <= 64 ? 64 : 128;
+    const size_t smem = (BN == 64 ? PlCfg<64>::kSmem : PlCfg<128>::kSmem) + (a0->colsum ? 4 * (size_t)a0->Cout : 0);
+    EFFDET_REQUIRE(smem <= kPlSmemOptin, "conv_planes_multi: column sums of %d channels do not fit in shared memory", a0->Cout);
+    for (int l = 0; l < nlevels; ++l) {
+        const effdet_conv_planes_args* a = &levels[l];
+        EFFDET_REQUIRE(!(a->mask_planes && a->mask_bits), "conv_planes_multi: level %d passes both mask_planes and mask_bits", l);
+        EFFDET_REQUIRE(!a->y_mask || (a->y_planes && a->act == EFFDET_ACT_RELU),
+                       "conv_planes_multi: y_mask is written by a ReLU forward that stores planes (level %d)", l);
+    }
     EncodeTiledFn enc = encode_fn();
     if (!enc) return fail(EFFDET_ERR_UNSUPPORTED, "conv_planes_multi: cuTensorMapEncodeTiled unavailable");
     EFFDET_DEVICE(device);
@@ -411,11 +489,14 @@ extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, i
     for (int l = 0; l < nlevels; ++l) {
         const effdet_conv_planes_args* a = &levels[l];
         EFFDET_REQUIRE(a->x_planes && (a->y || a->y_planes), "conv_planes_multi: null tensor");
+        EFFDET_REQUIRE(a->B > 0 && a->H > 0 && a->W > 0 && (long long)a->B * a->H * a->W <= INT_MAX,
+                       "conv_planes_multi: a %dx%dx%d map has more than 2^31 - 1 pixels", a->B, a->H, a->W);
         EFFDET_REQUIRE(a->Cin == a0->Cin && a->Cout == a0->Cout && a->ksize == a0->ksize && a->act == a0->act && a->w_tc == a0->w_tc &&
                            a->bias == a0->bias && a->colsum == a0->colsum,
                        "conv_planes_multi: all levels must share weights, bias, channels and activation");
         EFFDET_REQUIRE(aligned16(a->x_planes) && aligned16(a->y) && aligned16(a->y_planes) && aligned16(a->mask_planes) &&
-                           aligned16(a->residual) && a->y_bstride % 4 == 0 && a->r_bstride % 4 == 0,
+                           aligned16(a->residual) && a->y_bstride % 4 == 0 && a->r_bstride % 4 == 0 &&
+                           (reinterpret_cast<uintptr_t>(a->y_mask) & 3u) == 0 && (reinterpret_cast<uintptr_t>(a->mask_bits) & 3u) == 0,
                        "conv_planes_multi: alignment");
         PlLevel& L = P.lv[l];
         L.B = a->B; L.H = a->H; L.W = a->W;
@@ -428,6 +509,8 @@ extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, i
         L.y = a->y; L.y_bstride = a->y_bstride;
         L.y_planes = (__nv_bfloat16*)a->y_planes;
         L.mask_planes = (const __nv_bfloat16*)a->mask_planes;
+        L.y_mask = (uint32_t*)a->y_mask;
+        L.mask_bits = (const uint32_t*)a->mask_bits;
         L.residual = a->residual; L.r_bstride = a->r_bstride;
         int s = planes_map(enc, &maps.x[l], const_cast<void*>(a->x_planes), a->B, a->H, a->W, a->Cin, ipitch, L.g);
         if (s) return s;
@@ -438,8 +521,6 @@ extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, i
     }
     const int taps = a0->ksize * a0->ksize;
     const int kpad = conv_tc_kpad(a0->Cin);
-    // 128 x 128 tiles at most: the accumulator lives in the consumer warpgroups' registers (64 per thread)
-    const int BN = a0->Cout <= 64 ? 64 : 128;
     CUtensorMap wmap;
     const int s = kmajor_planes_map(enc, &wmap, a0->w_tc, a0->Cout, taps * kpad, BN);
     if (s) return s;
@@ -449,14 +530,15 @@ extern "C" int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, i
     P.Cin = a0->Cin; P.Cout = a0->Cout; P.ksize = a0->ksize; P.act = a0->act;
     P.kblocks = kpad / 64;
     P.opitch = opitch;
+    P.mwords = (a0->Cout + 31) / 32;
     P.bias = a0->bias;
     P.colsum = a0->colsum;
     const int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
     cudaStream_t st = (cudaStream_t)stream;
     if (a0->tc_single) {
-        if (BN == 64) return launch_smem("conv_planes_kernel", conv_planes_kernel<64, 1>, grid, kPlThreads, PlCfg<64>::kSmem, st, maps, wmap, P);
-        return launch_smem("conv_planes_kernel", conv_planes_kernel<128, 1>, grid, kPlThreads, PlCfg<128>::kSmem, st, maps, wmap, P);
+        if (BN == 64) return launch_smem("conv_planes_kernel", conv_planes_kernel<64, 1>, grid, kPlThreads, smem, st, maps, wmap, P);
+        return launch_smem("conv_planes_kernel", conv_planes_kernel<128, 1>, grid, kPlThreads, smem, st, maps, wmap, P);
     }
-    if (BN == 64) return launch_smem("conv_planes_kernel", conv_planes_kernel<64, 3>, grid, kPlThreads, PlCfg<64>::kSmem, st, maps, wmap, P);
-    return launch_smem("conv_planes_kernel", conv_planes_kernel<128, 3>, grid, kPlThreads, PlCfg<128>::kSmem, st, maps, wmap, P);
+    if (BN == 64) return launch_smem("conv_planes_kernel", conv_planes_kernel<64, 3>, grid, kPlThreads, smem, st, maps, wmap, P);
+    return launch_smem("conv_planes_kernel", conv_planes_kernel<128, 3>, grid, kPlThreads, smem, st, maps, wmap, P);
 }

@@ -97,7 +97,7 @@ class ConvPlanesArgs(ctypes.Structure):
     _fields_ = [('x_planes', _P), ('w_tc', _P), ('bias', _P), ('y', _P), ('y_bstride', _I64), ('y_planes', _P),
                 ('mask_planes', _P), ('residual', _P), ('r_bstride', _I64), ('colsum', _P),
                 ('B', _I32), ('H', _I32), ('W', _I32), ('Cin', _I32), ('Cout', _I32), ('ksize', _I32), ('act', _I32),
-                ('tc_single', _I32)]
+                ('tc_single', _I32), ('y_mask', _P), ('mask_bits', _P)]
 
 
 class DwFwdArgs(ctypes.Structure):

@@ -824,6 +824,11 @@ def _planes(B, H, W, C, like):
     return torch.empty((2, B, H, W, _pitch8(C)), device=like.device, dtype=torch.bfloat16)
 
 
+def _relu_bits(B, H, W, C, like):
+    """one bit per channel of a ReLU layer's planes (bit c % 32 of word c // 32: stored value > 0)"""
+    return torch.empty((B, H, W, (C + 31) // 32), device=like.device, dtype=torch.int32)
+
+
 def to_planes(x_ptr, x_bs, planes, B, HW, C, dev_t, prob_ptr=None, p_bs=0, colsum=None):
     N.call('effdet_to_planes', dev_t, x_ptr, x_bs, prob_ptr, p_bs, N.ptr(planes), N.f32(colsum, 'colsum'), B, HW, C,
            nbytes=8.0 * B * HW * C)
@@ -831,13 +836,14 @@ def to_planes(x_ptr, x_bs, planes, B, HW, C, dev_t, prob_ptr=None, p_bs=0, colsu
 
 def conv_planes_multi(dev_t, levels, w_tc, Cin, Cout, k, bias=None, act=ACT_NONE, colsum=None):
     """One launch over the pyramid levels; levels: dicts with x (planes), B, H, W and y_planes and / or (y_ptr, y_bs),
-    optional mask (planes), res_ptr / res_bs."""
+    optional y_mask (_relu_bits the ReLU forward writes), mask (planes) or mask_bits (a y_mask), res_ptr / res_bs."""
     nl = len(levels)
     arr = (N.ConvPlanesArgs * nl)()
     for i, lv in enumerate(levels):
         arr[i] = N.ConvPlanesArgs(N.ptr(lv['x']), w_tc.data_ptr(), N.f32(bias, 'bias'), lv.get('y_ptr'), lv.get('y_bs', 0),
                                   N.ptr(lv.get('y_planes')), N.ptr(lv.get('mask')), lv.get('res_ptr'), lv.get('res_bs', 0),
-                                  N.f32(colsum, 'colsum'), lv['B'], lv['H'], lv['W'], Cin, Cout, k, act, tc_single(k))
+                                  N.f32(colsum, 'colsum'), lv['B'], lv['H'], lv['W'], Cin, Cout, k, act, tc_single(k),
+                                  N.ptr(lv.get('y_mask')), N.ptr(lv.get('mask_bits')))
     px = sum(lv['B'] * lv['H'] * lv['W'] for lv in levels)
     N.call('effdet_conv_planes_multi', dev_t, arr, nl, flops=2.0 * px * k * k * Cin * Cout,
            nbytes=4.0 * (px * (Cin + Cout) + k * k * Cin * Cout))
@@ -889,24 +895,28 @@ class RetinaHeadPlanesFn(torch.autograd.Function):
             pl = _planes(f.shape[0], f.shape[1], f.shape[2], Cin, f)
             to_planes(N.f32(f), f.shape[1] * f.shape[2] * Cin, pl, f.shape[0], f.shape[1] * f.shape[2], Cin, dev_t)
             fp.append(pl)
-        towers = []
+        towers, tower_bits = [], []
         for tp in (cls_p, reg_p):
-            acts = [fp]
+            acts, bits = [fp], [None]                      # bits[i]: the ReLU mask of acts[i], for the data gradient
             cur, ci = fp, Cin
             for i in range(stacked):
                 nxt = [_planes(b, h, w, F, dev_t) for (b, h, w) in geo]
-                conv_planes_multi(dev_t, [dict(x=cur[l], y_planes=nxt[l], B=geo[l][0], H=geo[l][1], W=geo[l][2]) for l in range(nl)],
+                nbits = [_relu_bits(b, h, w, F, dev_t) for (b, h, w) in geo]
+                conv_planes_multi(dev_t, [dict(x=cur[l], y_planes=nxt[l], y_mask=nbits[l], B=geo[l][0], H=geo[l][1], W=geo[l][2])
+                                          for l in range(nl)],
                                   tc_packs(tp[2 * i])[0], ci, F, 3, bias=tp[2 * i + 1].detach(), act=ACT_RELU)
                 acts.append(nxt)
+                bits.append(nbits)
                 cur, ci = nxt, F
             towers.append(acts)
+            tower_bits.append(bits)
         for (acts, w, bias, out, width, act) in ((towers[0], wc, bc, cls_all, K, ACT_SIGMOID),
                                                  (towers[1], wr, br, reg_all, 4, ACT_NONE)):
             levels = [dict(x=acts[stacked][l], y_ptr=N.f32(out) + 4 * offs[l] * width, y_bs=tot * width, B=geo[l][0], H=geo[l][1],
                            W=geo[l][2]) for l in range(nl)]
             conv_planes_multi(dev_t, levels, tc_packs(w)[0], F, A * width, 3, bias=bias.detach(), act=act)
         ctx.meta = (nl, A, K, stacked, offs, tot, geo, Cin, F)
-        ctx.keep = (P, towers, cls_all)
+        ctx.keep = (P, towers, tower_bits, cls_all)
         return cls_all, reg_all
 
     @staticmethod
@@ -914,7 +924,7 @@ class RetinaHeadPlanesFn(torch.autograd.Function):
         nl, A, K, stacked, offs, tot, geo, Cin, F = ctx.meta
         if ctx.keep is None:
             raise RuntimeError('RetinaHeadPlanesFn: backward called twice (activations are released after the first backward)')
-        P, towers, cls_all = _stash(ctx, 'keep')
+        P, towers, tower_bits, cls_all = _stash(ctx, 'keep')
         cls_p, reg_p = P[:2 * stacked], P[2 * stacked:4 * stacked]
         wc, bc, wr, br = P[4 * stacked:4 * stacked + 4]
         dcls, dreg = _contig(dcls), _contig(dreg)
@@ -923,8 +933,9 @@ class RetinaHeadPlanesFn(torch.autograd.Function):
         g_cls, g_reg = gP[:2 * stacked], gP[2 * stacked:4 * stacked]
         gwc, gbc, gwr, gbr = gP[4 * stacked:4 * stacked + 4]
         dfeat = None
-        for (acts, tp, tg, wl, gwl, gbl, dsrc, prob, width) in ((towers[0], cls_p, g_cls, wc, gwc, gbc, dcls, cls_all, K),
-                                                               (towers[1], reg_p, g_reg, wr, gwr, gbr, dreg, None, 4)):
+        for (acts, bits, tp, tg, wl, gwl, gbl, dsrc, prob, width) in (
+                (towers[0], tower_bits[0], cls_p, g_cls, wc, gwc, gbc, dcls, cls_all, K),
+                (towers[1], tower_bits[1], reg_p, g_reg, wr, gwr, gbr, dreg, None, 4)):
             Co = A * width
             # gradient w.r.t. the head outputs -> planes (sigmoid backward folded in) + bias gradient of the output conv
             d = []
@@ -937,7 +948,7 @@ class RetinaHeadPlanesFn(torch.autograd.Function):
             wgrad_planes_multi(dev_t, [dict(x=top[l], dy=d[l], B=geo[l][0], H=geo[l][1], W=geo[l][2]) for l in range(nl)],
                                gwl, F, Co, 3)
             nxt = [_planes(b, h, w, F, dev_t) for (b, h, w) in geo]
-            conv_planes_multi(dev_t, [dict(x=d[l], y_planes=nxt[l], mask=top[l], B=geo[l][0], H=geo[l][1], W=geo[l][2])
+            conv_planes_multi(dev_t, [dict(x=d[l], y_planes=nxt[l], mask_bits=bits[stacked][l], B=geo[l][0], H=geo[l][1], W=geo[l][2])
                                       for l in range(nl)], tc_packs(wl)[1], Co, F, 3, colsum=tg[2 * (stacked - 1) + 1])
             d = nxt
             for i in range(stacked - 1, -1, -1):
@@ -948,7 +959,7 @@ class RetinaHeadPlanesFn(torch.autograd.Function):
                 wdt = tc_packs(tp[2 * i])[1]
                 if i > 0:
                     nxt = [_planes(b, h, w, F, dev_t) for (b, h, w) in geo]
-                    conv_planes_multi(dev_t, [dict(x=d[l], y_planes=nxt[l], mask=xin[l], B=geo[l][0], H=geo[l][1], W=geo[l][2])
+                    conv_planes_multi(dev_t, [dict(x=d[l], y_planes=nxt[l], mask_bits=bits[i][l], B=geo[l][0], H=geo[l][1], W=geo[l][2])
                                               for l in range(nl)], wdt, F, F, 3, colsum=tg[2 * (i - 1) + 1])
                     d = nxt
                 else:

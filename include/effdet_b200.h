@@ -129,7 +129,11 @@ int effdet_conv2d_wgrad_multi(const effdet_wgrad_args* levels, int nlevels, int 
  *   epilogue: v = acc + bias; v = act(v); v += residual; v = mask > 0 ? v : 0; store planes and / or fp32;
  *             colsum[n] += sum over pixels of v   (the bias gradient of the layer that produced this layer's input
  *             gradient -- a data-gradient launch hands it over for free)
- * Needs effdet_wgrad_tc_geometry_ok(B,H,W) for every level.
+ * The mask is given either as the forward's planes (mask_planes) or as the bits a ReLU forward wrote (mask_bits), not
+ * both.  y_mask / mask_bits: uint32 [B][H][W][(Cout + 31) / 32], bit c % 32 of word c / 32 set <=> the value stored in
+ * the planes for channel c is > 0 (words past Cout's last channel are zero).
+ * Needs effdet_wgrad_tc_geometry_ok(B,H,W) for every level; with colsum, 4 * Cout bytes of shared memory beyond the
+ * kernel's own (Cout up to about 3200).
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
     const void* x_planes;                       /* [2][B][H][W][pitch(Cin)] bf16 */
@@ -143,6 +147,8 @@ typedef struct {
     int32_t B, H, W, Cin, Cout, ksize, act;
     int32_t tc_single;                          /* 1: one bf16 product per multiply-add (hi planes only), as in
                                                    effdet_conv_args; 3x3 only, the same on every level */
+    void* y_mask;                               /* ReLU bits of the stored planes (act RELU with y_planes) or NULL */
+    const void* mask_bits;                      /* ReLU-backward mask as y_mask wrote it, or NULL */
 } effdet_conv_planes_args;
 int effdet_conv_planes_multi(const effdet_conv_planes_args* levels, int nlevels, int device, effdet_stream_t stream);
 /* fp32 [B][HW][C] (image stride x_bstride) -> planes [2][B*HW][pitch(C)]; with prob != NULL the value is first
