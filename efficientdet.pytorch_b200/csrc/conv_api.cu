@@ -8,8 +8,9 @@ int pw_gemm_launch(const effdet_conv_args* a, cudaStream_t st);                 
 int conv_tc_launch(const effdet_conv_args* levels, int nlevels, cudaStream_t st);      // conv_tc.cu
 int conv_simt_launch(const effdet_conv_args* a, cudaStream_t st);                      // conv_simt.cu
 int pw_wgrad_launch(const effdet_wgrad_args* a, cudaStream_t st);                      // pw_wgrad.cu
-int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t st);   // conv_tc.cu
-int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st);                      // conv_tc.cu
+int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, float* acc, cudaStream_t st);   // conv_tc.cu
+int wgrad_tc_launch(const effdet_wgrad_args* a, float* acc, cudaStream_t st);                      // conv_tc.cu
+int wgrad_fold_launch(const float* ws, float* dw, long long nc, cudaStream_t st);                  // conv_tc.cu
 int wgrad_simt_launch(const effdet_wgrad_args* a, cudaStream_t st);                    // conv_simt.cu
 int colsum_launch(const float* x, float* out, long long M, int N, long long HW, long long bstride, cudaStream_t st);  // conv_simt.cu
 
@@ -55,14 +56,15 @@ static int conv_level(const effdet_conv_args* a, cudaStream_t st) {
     return conv_simt_launch(a, st);
 }
 
-// the bias gradient comes from the dy split pass on the TMA-fed route, from a column sum on the others
-static int wgrad_level(const effdet_wgrad_args* a, cudaStream_t st) {
+// the bias gradient comes from the dy split pass on the TMA-fed route, from a column sum on the others; the tensor-core
+// kernels add into acc ([taps][Cout][Cin]), the others into dw
+static int wgrad_level(const effdet_wgrad_args* a, float* acc, cudaStream_t st) {
     if (pw_wgrad_eligible(a)) return pw_wgrad_launch(a, st);
-    if (wgrad_tma_eligible(a)) return wgrad_tc2_launch(a, 1, st);
+    if (wgrad_tma_eligible(a)) return wgrad_tc2_launch(a, 1, acc, st);
     if (a->dy_planes || a->x_planes)                  // the other kernels read fp32 operands only
         return fail(EFFDET_ERR_UNSUPPORTED, "wgrad: dy_planes given but the TMA-fed tensor-core kernel cannot take this shape or "
                                             "input prologue (check effdet_wgrad_tc_geometry_ok first)");
-    const int s = wgrad_tc_eligible(a) ? wgrad_tc_launch(a, st) : wgrad_simt_launch(a, st);
+    const int s = wgrad_tc_eligible(a) ? wgrad_tc_launch(a, acc, st) : wgrad_simt_launch(a, st);
     if (s || !a->dbias) return s;
     return colsum_launch(a->dy, a->dbias, (long long)a->B * a->H * a->W, a->Cout, (long long)a->H * a->W, a->dy_bstride, st);
 }
@@ -106,7 +108,8 @@ static int check_wgrad_level(const effdet_wgrad_args* a, const effdet_wgrad_args
     EFFDET_REQUIRE(!a->tc_single || a->ksize == 3, "wgrad: tc_single is defined for 3x3 convolutions only (ksize %d)", a->ksize);
     EFFDET_REQUIRE(a->Cin % 4 == 0 && a->Cout % 4 == 0, "wgrad: channels must be multiples of 4");
     EFFDET_REQUIRE(a->B > 0 && a->H > 0 && a->W > 0, "wgrad: empty shape");
-    EFFDET_REQUIRE(aligned16(a->x) && aligned16(a->dy) && aligned16(a->a_scale) && aligned16(a->in_scale) && aligned16(a->in_shift),
+    EFFDET_REQUIRE(aligned16(a->x) && aligned16(a->dy) && aligned16(a->dw) && aligned16(a->a_scale) && aligned16(a->in_scale) &&
+                       aligned16(a->in_shift) && aligned16(a->ws_dw),
                    "wgrad: pointers must be 16-byte aligned");
     EFFDET_REQUIRE((a->in_scale == nullptr) == (a->in_shift == nullptr) && (!a->in_scale || a->ksize == 1),
                    "wgrad: in_scale/in_shift must come together (1x1 convs only)");
@@ -137,13 +140,28 @@ static int conv2d_wgrad(const effdet_wgrad_args* levels, int nlevels, int device
     EFFDET_REQUIRE(nlevels >= 1, "conv2d_wgrad_multi: no levels");
     for (int l = 0; l < nlevels; ++l)
         if (const int s = check_wgrad_level(levels + l, levels)) return s;
+    // the tensor-core kernels reduce into a tap-major [taps][Cout][Cin] accumulator: dw itself for a 1x1 conv, the first
+    // level's ws_dw for a 3x3 one, which is cleared here and folded into dw after the launches
+    const effdet_wgrad_args* a0 = levels;
+    bool tc3 = false;
+    for (int l = 0; l < nlevels; ++l) tc3 = tc3 || (a0->ksize == 3 && wgrad_tc_eligible(&levels[l]));
+    EFFDET_REQUIRE(!tc3 || a0->ws_dw, "wgrad: a 3x3 tensor-core weight gradient needs the ws_dw workspace (4*9*Cout*Cin bytes)");
     EFFDET_DEVICE(device);
+    const long long nc = (long long)a0->Cout * a0->Cin;
+    float* acc = tc3 ? static_cast<float*>(a0->ws_dw) : a0->dw;
+    if (tc3) {
+        const cudaError_t e = cudaMemsetAsync(acc, 0, 9 * nc * sizeof(float), st);
+        if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "wgrad: clearing ws_dw: %s", cudaGetErrorString(e));
+    }
     bool one = nlevels > 1 && nlevels <= kWgMaxLevels;      // one level keeps its own route, the pointwise kernel included
     for (int l = 0; l < nlevels; ++l) one = one && wgrad_tma_eligible(&levels[l]);
-    if (one) return wgrad_tc2_launch(levels, nlevels, st);
     int s = EFFDET_OK;
-    for (int l = 0; l < nlevels && !s; ++l) s = wgrad_level(&levels[l], st);
-    return s;
+    if (one)
+        s = wgrad_tc2_launch(levels, nlevels, acc, st);
+    else
+        for (int l = 0; l < nlevels && !s; ++l) s = wgrad_level(&levels[l], acc, st);
+    if (s || !tc3) return s;
+    return wgrad_fold_launch(acc, a0->dw, nc, st);
 }
 
 }  // namespace effdet

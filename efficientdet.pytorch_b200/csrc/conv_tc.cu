@@ -23,7 +23,9 @@
 //              sigmoid / ReLU-mask / residual, 128-bit stores straight into the caller's layout)
 //   warp 8     TMA: weight tiles (pre-split bf16 planes) -> smem, mbarrier complete_tx
 // Weight gradient: both operands are NHWC rows (pixels are the GEMM-K dimension, so they are
-// MN-major operands), split-K over pixel ranges with fp32 atomics into the OIHW gradient.
+// MN-major operands), split-K over pixel ranges with fp32 vector reductions into a tap-major accumulator
+// [taps][Cout][Cin] (for a 3x3 conv a workspace that wgrad_fold_kernel adds into the OIHW gradient, for a 1x1 conv the
+// gradient itself).
 #include "tc_ptx.cuh"
 
 namespace effdet {
@@ -241,7 +243,8 @@ struct WgSmem {
     static constexpr int kA = kTileK * 128 * (kTileM / 64);   // one plane of the dy tile: 2 channel groups
     static constexpr int kB = kTileK * 128 * (BC / 64);       // one plane of the x tile
     static constexpr int kStage = 2 * kA + 2 * kB;
-    static constexpr int kBytes = STAGES * kStage + 1024 + 256;
+    static constexpr int kXch = STAGES * kStage + 256;        // the epilogue's lane exchange: 2 x 32 float2 per warp
+    static constexpr int kBytes = kXch + 8 * 2 * 32 * 8 + 1024;
 };
 
 // gather `ngroups` channel groups (64 channels each) of 64 pixel rows into swizzled bf16 planes (NP = 1: hi plane only)
@@ -284,25 +287,45 @@ __device__ __forceinline__ void wg_produce(const float* __restrict__ src, const 
     }
 }
 
-// fp32 atomics of a warpgroup's accumulator (64 output channels from n0 x NB*64 input channels from c0) into the OIHW
-// weight gradient
+__device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+
+// Adds a warpgroup's accumulator (64 output channels from n0 x NB*64 input channels from c0) into the tap-major fp32
+// accumulator acc[taps][Cout][Cin], where input channels are contiguous.  In the wgmma fragment a lane holds columns 2q,
+// 2q+1 of rows r and r+8 in each 8-column block; lanes 2k and 2k+1 swap one pair so that the even lane holds 4
+// consecutive columns of row r and the odd lane 4 of row r+8, and each issues one 16-byte vector reduction.
+// Cin % 4 == 0, so a 4-column group lies wholly inside or wholly outside Cin.
+// The swap goes through the warp's 64 float2 of shared memory (xch, two slots per lane used in turn, so one __syncwarp
+// per block orders both the reuse and the read): a warp shuffle in the consumer branch of wgrad_tc2_multi_kernel makes
+// ptxas serialize that kernel's wgmma (C7520).
 template <int NB>
-__device__ __forceinline__ void wg_atomic_dw(const float (&d)[NB][32], float* dw, const int n0, const int c0, const int Cout,
-                                             const int Cin, const int kk, const int tap) {
+__device__ __forceinline__ void wg_red_dw(const float (&d)[NB][32], float* acc, const int n0, const int c0, const int Cout,
+                                          const int Cin, const int tap, float2* xch) {
     const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const bool odd = lane & 1;
+    const int n = n0 + 16 * w + (lane >> 2) + 8 * odd;
+    float* row = acc + ((long long)tap * Cout + n) * Cin + c0 + 2 * (lane & 2);
 #pragma unroll
     for (int jb = 0; jb < NB; ++jb)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-            const int n = n0 + 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);
-            const int c = c0 + jb * 64 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-            if (n < Cout && c < Cin) atomicAdd(dw + ((long long)n * Cin + c) * kk + tap, d[jb][i]);
+        for (int b = 0; b < 8; ++b) {
+            const float* v = &d[jb][4 * b];      // (r, 2q), (r, 2q+1), (r+8, 2q), (r+8, 2q+1)
+            float2* slot = xch + 32 * (b & 1);
+            slot[lane] = odd ? make_float2(v[0], v[1]) : make_float2(v[2], v[3]);
+            __syncwarp();
+            const float2 t = slot[lane ^ 1];
+            const float s0 = t.x, s1 = t.y;
+            const float x0 = odd ? s0 : v[0], x1 = odd ? s1 : v[1], x2 = odd ? v[2] : s0, x3 = odd ? v[3] : s1;
+            const int c = c0 + jb * 64 + 8 * b + 2 * (lane & 2);
+            if (n < Cout && c < Cin) red_add_v4(row + jb * 64 + 8 * b, x0, x1, x2, x3);
         }
 }
 
 template <int BC, int STAGES, int NP>
 __global__ void __launch_bounds__(kTcProducers, 1)
-wgrad_tc_kernel(const __grid_constant__ WgradPrefix pa, const int M, const int HW, const int chunks_per_split, const int ctiles) {
+wgrad_tc_kernel(const __grid_constant__ WgradPrefix pa, float* acc, const int M, const int HW, const int chunks_per_split,
+                const int ctiles) {
     using S = WgSmem<BC, STAGES>;
     const effdet_wgrad_args& p = pa.get();
     extern __shared__ uint8_t smem_raw[];
@@ -338,8 +361,8 @@ wgrad_tc_kernel(const __grid_constant__ WgradPrefix pa, const int M, const int H
         wgmma_commit();
     }
     wgmma_wait<0>();
-    // epilogue: row = output channel n, columns = input channels c -> atomics into OIHW
-    wg_atomic_dw<NB>(d, p.dw, n0 + 64 * g, c0, p.Cout, p.Cin, p.ksize * p.ksize, tap);
+    // epilogue: row = output channel n, columns = input channels c -> vector reductions into acc[tap][n][c]
+    wg_red_dw<NB>(d, acc, n0 + 64 * g, c0, p.Cout, p.Cin, tap, reinterpret_cast<float2*>(smem + S::kXch) + 64 * warp);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -348,7 +371,7 @@ wgrad_tc_kernel(const __grid_constant__ WgradPrefix pa, const int M, const int H
 // disappear: one thread issues 5-D tensor-map loads (channel group, x, y, image, plane) whose
 // out-of-bounds zero fill IS the convolution's zero padding (the tap shift is just a coordinate
 // offset); two consumer warpgroups (64 output channels each) issue the wgmma and add their
-// accumulators to the OIHW gradient with atomics.  A stage covers a box of
+// accumulators to the tap-major accumulator with vector reductions.  A stage covers a box of
 // kstage = Wb*Hb*Bb pixels (<= 64, multiple of 16).
 // The pixel chunks of several pyramid levels (same weights, e.g. the five RetinaHead levels) form
 // one long GEMM-K dimension, so one launch covers them all; each chunk looks up its level's tensor
@@ -362,7 +385,7 @@ struct WgMultiArgs {
     WgGeom g[kWgMaxLevels];
     int chunk_begin[kWgMaxLevels + 1];
     int nlevels;
-    float* dw;
+    float* acc;          // [taps][Cout][Cin]
     int Cin, Cout, ksize;
 };
 
@@ -450,8 +473,24 @@ wgrad_tc2_multi_kernel(const __grid_constant__ WgMaps maps, const __grid_constan
             });
         }
         wgmma_wait<0>();
-        wg_atomic_dw<NB>(d, a.dw, n0 + 64 * wg, c0, a.Cout, a.Cin, a.ksize * a.ksize, tap);
+        wg_red_dw<NB>(d, a.acc, n0 + 64 * wg, c0, a.Cout, a.Cin, tap, reinterpret_cast<float2*>(smem + S::kXch) + 64 * warp);
     }
+}
+
+// Adds the tap-major accumulator of a 3x3 weight gradient into the OIHW gradient: dw[n][c][tap] += ws[tap][n][c].
+// A CTA takes kFoldPairs consecutive (n, c) pairs, reads their 9 tap rows coalesced, transposes them through shared
+// memory (stride 9, odd: no bank conflicts) and adds them to the 9 * kFoldPairs consecutive floats of dw they map to.
+constexpr int kFoldPairs = 256;
+__global__ void __launch_bounds__(kFoldPairs)
+wgrad_fold_kernel(const float* __restrict__ ws, float* __restrict__ dw, const long long nc) {
+    __shared__ float t[9 * kFoldPairs];
+    const long long j0 = (long long)blockIdx.x * kFoldPairs;
+    const int np = (int)min((long long)kFoldPairs, nc - j0);
+    if (threadIdx.x < np)
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) t[threadIdx.x * 9 + tap] = __ldg(ws + tap * nc + j0 + threadIdx.x);
+    __syncthreads();
+    for (int i = threadIdx.x; i < 9 * np; i += kFoldPairs) dw[j0 * 9 + i] += t[i];
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -579,7 +618,7 @@ int planes_map(EncodeTiledFn enc, CUtensorMap* map, void* base, int B, int H, in
 
 // TMA-fed weight gradient of one shared-weight layer over all levels in one launch.  conv_api.cu has checked that every
 // level has a pixel box and both operands as planes or plane workspaces, and that the tensor-map encoder is available.
-int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t st) {
+int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, float* acc, cudaStream_t st) {
     EncodeTiledFn enc = encode_fn();
     WgMaps maps;
     WgMultiArgs ma;
@@ -595,7 +634,7 @@ int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t 
     }
     for (int l = nlevels; l <= kWgMaxLevels; ++l) ma.chunk_begin[l] = chunks;
     ma.nlevels = nlevels;
-    ma.dw = a0->dw;
+    ma.acc = acc;
     ma.Cin = a0->Cin; ma.Cout = a0->Cout; ma.ksize = a0->ksize;
     for (int l = 0; l < nlevels; ++l) {
         const effdet_wgrad_args* a = &levels[l];
@@ -645,7 +684,7 @@ int wgrad_tc2_launch(const effdet_wgrad_args* levels, int nlevels, cudaStream_t 
 }
 
 // weight gradient of one level from fp32 operands that the kernel gathers itself; the bias gradient is not part of it
-int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st) {
+int wgrad_tc_launch(const effdet_wgrad_args* a, float* acc, cudaStream_t st) {
     const int M = a->B * a->H * a->W, HW = a->H * a->W;
     const int taps = a->ksize * a->ksize;
     const int BC = a->Cin > 64 ? 256 : 64;
@@ -662,15 +701,22 @@ int wgrad_tc_launch(const effdet_wgrad_args* a, cudaStream_t st) {
     pa.set(*a);
     if (a->tc_single) {
         if (BC == 256)
-            return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<256, 2, 1>, grid, kTcProducers, WgSmem<256, 2>::kBytes, st, pa, M, HW,
-                               cps, ctiles);
-        return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<64, 4, 1>, grid, kTcProducers, WgSmem<64, 4>::kBytes, st, pa, M, HW, cps,
-                           ctiles);
+            return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<256, 2, 1>, grid, kTcProducers, WgSmem<256, 2>::kBytes, st, pa,
+                               acc, M, HW, cps, ctiles);
+        return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<64, 4, 1>, grid, kTcProducers, WgSmem<64, 4>::kBytes, st, pa, acc, M,
+                           HW, cps, ctiles);
     }
     if (BC == 256)
-        return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<256, 2, 3>, grid, kTcProducers, WgSmem<256, 2>::kBytes, st, pa, M, HW, cps,
-                           ctiles);
-    return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<64, 4, 3>, grid, kTcProducers, WgSmem<64, 4>::kBytes, st, pa, M, HW, cps, ctiles);
+        return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<256, 2, 3>, grid, kTcProducers, WgSmem<256, 2>::kBytes, st, pa, acc, M,
+                           HW, cps, ctiles);
+    return launch_smem("wgrad_tc_kernel", wgrad_tc_kernel<64, 4, 3>, grid, kTcProducers, WgSmem<64, 4>::kBytes, st, pa, acc, M, HW,
+                       cps, ctiles);
+}
+
+// dw[n][c][tap] += ws[tap][n][c] for the nc = Cout * Cin (n, c) pairs of a 3x3 weight gradient
+int wgrad_fold_launch(const float* ws, float* dw, long long nc, cudaStream_t st) {
+    wgrad_fold_kernel<<<cdiv(nc, kFoldPairs), kFoldPairs, 0, st>>>(ws, dw, nc);
+    return launch_status("wgrad_fold_kernel");
 }
 
 }  // namespace effdet

@@ -84,7 +84,7 @@ class WgradArgs(ctypes.Structure):
     _fields_ = [('x', _P), ('x_bstride', _I64), ('dy', _P), ('dy_bstride', _I64), ('dw', _P), ('dbias', _P),
                 ('a_scale', _P), ('B', _I32), ('H', _I32), ('W', _I32), ('Cin', _I32), ('Cout', _I32), ('ksize', _I32),
                 ('precision', _I32), ('ws_x', _P), ('ws_dy', _P), ('in_scale', _P), ('in_shift', _P), ('dy_planes', _P),
-                ('x_planes', _P), ('tc_single', _I32)]
+                ('x_planes', _P), ('tc_single', _I32), ('ws_dw', _P)]
 
 
 class BnActBwdArgs(ctypes.Structure):

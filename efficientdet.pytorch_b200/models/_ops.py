@@ -279,10 +279,16 @@ def conv2d_multi(xs, wf, Cout, k, bias=None, act=ACT_NONE, w_tc=None, residuals=
     return ys
 
 
+def _ws_dw(dev_t, Cin, Cout, k):
+    """the fp32 [9][Cout][Cin] workspace a 3x3 tensor-core weight gradient reduces into (1x1: None, dw itself)"""
+    return torch.empty((9 * Cout * Cin,), device=dev_t.device, dtype=torch.float32) if k == 3 else None
+
+
 def conv_wgrad_raw(dev_t, x_ptr, x_bs, dy_ptr, dy_bs, dw, dbias, B, H, W, Cin, Cout, k, a_scale=None, tc=False,
                    in_scale=None, in_shift=None, dy_planes=None):
-    ws_x = ws_dy = None
+    ws_x = ws_dy = ws_dw = None
     if tc:
+        ws_dw = _ws_dw(dev_t, Cin, Cout, k)
         lib = N.load()
         ws_x = torch.empty((2 * B * H * W * lib.effdet_conv_tc_kpad(Cin),), device=dev_t.device, dtype=torch.bfloat16)
         if dy_planes is None:
@@ -290,7 +296,8 @@ def conv_wgrad_raw(dev_t, x_ptr, x_bs, dy_ptr, dy_bs, dw, dbias, B, H, W, Cin, C
     a = N.WgradArgs(x_ptr, x_bs, dy_ptr, dy_bs, N.f32(dw, 'dw'), N.f32(dbias, 'dbias'), N.f32(a_scale, 'a_scale'),
                     B, H, W, Cin, Cout, k, 1 if tc else 0, ws_x.data_ptr() if ws_x is not None else None,
                     ws_dy.data_ptr() if ws_dy is not None else None, N.f32(in_scale, 'in_scale'),
-                    N.f32(in_shift, 'in_shift'), N.ptr(dy_planes), None, tc_single(k) if tc else 0)
+                    N.f32(in_shift, 'in_shift'), N.ptr(dy_planes), None, tc_single(k) if tc else 0,
+                    ws_dw.data_ptr() if ws_dw is not None else None)
     N.call('effdet_conv2d_wgrad', dev_t, a)
 
 
@@ -313,6 +320,7 @@ def conv_wgrad_multi(dev_t, levels, dw, dbias, Cin, Cout, k, tc=False):
     keep = []
     lib = N.load()
     kin, kout = lib.effdet_conv_tc_kpad(Cin), lib.effdet_conv_tc_kpad(Cout)
+    ws_dw = _ws_dw(dev_t, Cin, Cout, k) if tc else None
     for i, lv in enumerate(levels):
         ws_x = ws_dy = None
         if tc:
@@ -323,7 +331,7 @@ def conv_wgrad_multi(dev_t, levels, dw, dbias, Cin, Cout, k, tc=False):
         arr[i] = N.WgradArgs(lv['x_ptr'], lv['x_bs'], lv['dy_ptr'], lv['dy_bs'], N.f32(dw, 'dw'), N.f32(dbias, 'dbias'),
                              None, lv['B'], lv['H'], lv['W'], Cin, Cout, k, 1 if tc else 0,
                              ws_x.data_ptr() if ws_x is not None else None, ws_dy.data_ptr() if ws_dy is not None else None,
-                             tc_single=tc_single(k) if tc else 0)
+                             tc_single=tc_single(k) if tc else 0, ws_dw=ws_dw.data_ptr() if ws_dw is not None else None)
     N.call('effdet_conv2d_wgrad_multi', dev_t, arr, nl)
 
 
@@ -854,9 +862,11 @@ def wgrad_planes_multi(dev_t, levels, dw, Cin, Cout, k):
     levels: dicts with x (planes), dy (planes), B, H, W."""
     nl = len(levels)
     arr = (N.WgradArgs * nl)()
+    ws_dw = _ws_dw(dev_t, Cin, Cout, k)
     for i, lv in enumerate(levels):
         arr[i] = N.WgradArgs(None, 0, None, 0, N.f32(dw, 'dw'), None, None, lv['B'], lv['H'], lv['W'], Cin, Cout, k, 1, None,
-                             None, None, None, N.ptr(lv['dy']), N.ptr(lv['x']), tc_single(k))
+                             None, None, None, N.ptr(lv['dy']), N.ptr(lv['x']), tc_single(k),
+                             ws_dw.data_ptr() if ws_dw is not None else None)
     N.call('effdet_conv2d_wgrad_multi', dev_t, arr, nl)
 
 

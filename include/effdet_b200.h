@@ -114,6 +114,10 @@ typedef struct {
                               fp32 accumulation) instead of bf16x3; 3x3 convolutions only (ksize 1 -> EFFDET_ERR_ARG).
                               0 keeps the bf16x3 split precision. Needs precision 1 (else EFFDET_ERR_ARG); every
                               level of a multi-level call must pass the same value */
+    void* ws_dw;           /* fp32 workspace of 4*9*Cout*Cin bytes, 16-byte aligned, that the tensor-core kernels of a 3x3
+                              weight gradient reduce into (tap-major [9][Cout][Cin]) before one fold adds it to dw; needed
+                              when a 3x3 call takes a tensor-core route, else unused.  A multi-level call uses the first
+                              level's.  1x1 tensor-core weight gradients reduce straight into dw */
 } effdet_wgrad_args;
 int effdet_conv2d_wgrad(const effdet_wgrad_args* a, int device, effdet_stream_t stream);
 /* Weight gradient of one shared-weight layer accumulated over `nlevels` feature maps in one launch (all levels
