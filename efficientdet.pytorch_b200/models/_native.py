@@ -154,6 +154,9 @@ SIGNATURES = {
     'effdet_bifpn_fuse_bwd': [ctypes.POINTER(FuseBwdArgs)] + _TAIL,
     'effdet_focal_loss_fwd': [_P] * 7 + [_INT] * 4 + [_F, _F] + _TAIL,
     'effdet_focal_loss_bwd': [_P] * 9 + [_INT] * 4 + [_F, _F] + _TAIL,
+    'effdet_focal_loss_counted_fwd': [_P] * 8 + [_INT] * 4 + [_F, _F] + _TAIL,
+    'effdet_focal_loss_counted_bwd': [_P] * 10 + [_INT] * 4 + [_F, _F] + _TAIL,
+    'effdet_pack_annots': [_P, _INT, _INT, _P, _P, _INT, _INT] + _TAIL,
     'effdet_sigmoid_bwd': [_P, _P, _P, _I64] + _TAIL,
     'effdet_detect_candidates_batch': [_P] * 8 + [_INT, _INT, _INT, _INT, _F, _F, _F] + _TAIL,
     'effdet_nms_batch': [_P, _P, _P, _INT, _INT, _INT, _INT, ctypes.c_double, _P, _P, _P] + _TAIL,

@@ -988,9 +988,25 @@ class RetinaHeadPlanesFn(torch.autograd.Function):
 # ------------------------------------------------------------------------------------------------
 
 
+# Annotation rows per image that effdet_focal_loss_fwd / _bwd stage in shared memory at once; wider tables, and calls
+# with device-side counts, go through the counted pair, which stages them in chunks of this many rows.
+FOCAL_MAX_G = 256
+
+
+def annotation_counts(B, G, device):
+    """[1 + B] int32 on the device: (B, G, ..., G), every image and every row.  Two fills, no host read."""
+    counts = torch.full((1 + B,), G, dtype=torch.int32, device=device)
+    counts[:1].fill_(B)
+    return counts
+
+
 class FocalLossFn(torch.autograd.Function):
+    """counts: None, or [1 + B] int32 on the device (include/effdet_b200.h, effdet_focal_loss_counted_fwd): counts[0]
+    real images (the loss is their mean), counts[1 + b] annotation rows of image b.  With counts, or with more than
+    FOCAL_MAX_G annotation rows, the counted entry points run; otherwise the uncounted pair."""
+
     @staticmethod
-    def forward(ctx, cls, reg, anchors, annots, alpha, gamma):
+    def forward(ctx, cls, reg, anchors, annots, alpha, gamma, counts=None):
         check_cuda_f32(cls, 'classifications')
         check_cuda_f32(reg, 'regressions')
         cls, reg = _contig(cls), _contig(reg)
@@ -998,19 +1014,34 @@ class FocalLossFn(torch.autograd.Function):
         annots = _contig(annots.to(device=cls.device, dtype=torch.float32))
         B, A, K = cls.shape
         G = annots.shape[1]
+        if (counts is not None or G > FOCAL_MAX_G) and tuple(annots.shape) != (B, G, 5):
+            raise N.EffdetNativeError('FocalLoss: annotations must be [B=%d, G, 5], got %s' % (B, tuple(annots.shape)))
+        if counts is not None:
+            if counts.dtype != torch.int32 or counts.numel() != 1 + B or counts.device != cls.device:
+                raise N.EffdetNativeError('FocalLoss: counts must be a [1 + B] = [%d] int32 tensor on %s, got %s %s on %s'
+                                          % (1 + B, cls.device, tuple(counts.shape), counts.dtype, counts.device))
+            counts = _contig(counts)
+        elif G > FOCAL_MAX_G:
+            counts = annotation_counts(B, G, cls.device)
         losses = _empty((2,), cls)
         assign = torch.empty((B, A), device=cls.device, dtype=torch.int32)
         stats = _empty((B, 4), cls)
-        N.call('effdet_focal_loss_fwd', cls, N.f32(cls), N.f32(reg), N.f32(anchors.view(-1, 4)), N.f32(annots),
-               N.f32(losses), assign.data_ptr(), N.f32(stats), B, A, K, G, float(alpha), float(gamma),
-               nbytes=4.0 * (cls.numel() + reg.numel()))
-        ctx.save_for_backward(cls, reg, anchors, annots, assign, stats)
+        if counts is None:
+            N.call('effdet_focal_loss_fwd', cls, N.f32(cls), N.f32(reg), N.f32(anchors.view(-1, 4)), N.f32(annots),
+                   N.f32(losses), assign.data_ptr(), N.f32(stats), B, A, K, G, float(alpha), float(gamma),
+                   nbytes=4.0 * (cls.numel() + reg.numel()))
+            ctx.save_for_backward(cls, reg, anchors, annots, assign, stats)
+        else:
+            N.call('effdet_focal_loss_counted_fwd', cls, N.f32(cls), N.f32(reg), N.f32(anchors.view(-1, 4)),
+                   N.f32(annots), N.ptr(counts), N.f32(losses), assign.data_ptr(), N.f32(stats), B, A, K, G, float(alpha),
+                   float(gamma), nbytes=4.0 * (cls.numel() + reg.numel()))
+            ctx.save_for_backward(cls, reg, anchors, annots, assign, stats, counts)
         ctx.hp = (float(alpha), float(gamma))
         return losses.narrow(0, 0, 1), losses.narrow(0, 1, 1)
 
     @staticmethod
     def backward(ctx, g_cls, g_reg):
-        cls, reg, anchors, annots, assign, stats = ctx.saved_tensors
+        cls, reg, anchors, annots, assign, stats, *counts = ctx.saved_tensors
         B, A, K = cls.shape
         G = annots.shape[1]
         gout = _zeros((2,), cls)
@@ -1019,10 +1050,23 @@ class FocalLossFn(torch.autograd.Function):
         if g_reg is not None:
             gout[1:2].copy_(g_reg.reshape(1))
         dcls, dreg = torch.empty_like(cls), torch.empty_like(reg)
-        N.call('effdet_focal_loss_bwd', cls, N.f32(cls), N.f32(reg), N.f32(anchors.view(-1, 4)), N.f32(annots),
-               N.f32(gout), assign.data_ptr(), N.f32(stats), N.f32(dcls), N.f32(dreg), B, A, K, G, ctx.hp[0], ctx.hp[1],
-               nbytes=8.0 * (cls.numel() + reg.numel()))
-        return dcls, dreg, None, None, None, None
+        if not counts:
+            N.call('effdet_focal_loss_bwd', cls, N.f32(cls), N.f32(reg), N.f32(anchors.view(-1, 4)), N.f32(annots),
+                   N.f32(gout), assign.data_ptr(), N.f32(stats), N.f32(dcls), N.f32(dreg), B, A, K, G, ctx.hp[0],
+                   ctx.hp[1], nbytes=8.0 * (cls.numel() + reg.numel()))
+        else:
+            N.call('effdet_focal_loss_counted_bwd', cls, N.f32(cls), N.f32(reg), N.f32(anchors.view(-1, 4)),
+                   N.f32(annots), N.ptr(counts[0]), N.f32(gout), assign.data_ptr(), N.f32(stats), N.f32(dcls),
+                   N.f32(dreg), B, A, K, G, ctx.hp[0], ctx.hp[1], nbytes=8.0 * (cls.numel() + reg.numel()))
+        return dcls, dreg, None, None, None, None, None
+
+
+def pack_annotations(annots, out, counts):
+    """Copy a ragged collated batch annots [B, G, 5] (-1 padded, B <= Bcap, G <= Gcap) into the static table out
+    [Bcap, Gcap, 5] and counts [1 + Bcap] (effdet_pack_annots): each image's labelled rows first, in order.  One launch,
+    no host read."""
+    B, G = annots.shape[0], annots.shape[1]
+    N.call('effdet_pack_annots', out, N.f32(annots), B, G, N.f32(out), N.ptr(counts), out.shape[0], out.shape[1])
 
 
 # ------------------------------------------------------------------------------------------------

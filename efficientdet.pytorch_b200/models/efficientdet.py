@@ -2,6 +2,8 @@
 around sm_90a kernels.  Same constructor, attributes, call convention and state-dict schema:
 
   train :  model([images[B,3,H,W], annotations[B,G,5]]) -> (cls_loss[1], reg_loss[1])   (reference :57-68)
+           model([images, annotations, counts[1+B] int32]) -> the same, over the first counts[0] images with counts[1+b]
+           annotation rows each (models/losses.py); the rest of the batch is padding
   eval  :  model(image[1,3,H,W]) -> [scores[K], classes[K] int64, boxes[K,4]]            (reference :69-86)
 
 What differs underneath: features stay NHWC end to end, the head writes the level-concatenated
@@ -84,9 +86,9 @@ class EfficientDet(nn.Module):
         cls, reg = self.bbox_head.forward_concat_nhwc(self.extract_feat_nhwc(images))
         return cls, reg, self.anchors(images)
 
-    def _losses(self, images, annotations):
+    def _losses(self, images, annotations, counts=None):
         cls, reg, anchors = self._raw_predictions(images)
-        return self.criterion(cls, reg, anchors, annotations)
+        return self.criterion(cls, reg, anchors, annotations, counts)
 
     def _detections(self, image):
         cls, reg, anchors = self._raw_predictions(image)
@@ -120,6 +122,9 @@ class EfficientDet(nn.Module):
 
     def forward(self, inputs):
         if self.is_training:
-            images, annotations = inputs
-            return self._losses(images, annotations)
+            images, annotations, *counts = inputs
+            if len(counts) > 1:
+                raise _ops.N.EffdetNativeError('EfficientDet: training inputs are [images, annotations] or '
+                                               '[images, annotations, counts], got %d elements' % len(inputs))
+            return self._losses(images, annotations, *counts)
         return self._detections(inputs)

@@ -18,9 +18,23 @@ Build it BEFORE any eager step, or after every reference to earlier eager losses
 graph keeps the parameters' gradient accumulators bound to the stream it ran on (the legacy stream), and the engine
 may not touch that stream while another one is capturing.
 
-Shapes are static (the reference pads every batch to the common size and a fixed annotation count per batch can be
-obtained by padding with -1 rows, which FocalLoss ignores).  Drop-connect keeps working: torch.rand inside a captured
-region advances the Philox offset on every replay.
+Shapes are static by default: every call takes images and annotations of the example's shapes.  Drop-connect keeps
+working: torch.rand inside a captured region advances the Philox offset on every replay.
+
+Capacity mode, for the batches a DataLoader with collate_fn=collater yields.  The collater pads each batch to the
+largest annotation count in THAT batch, and the last batch of an epoch is short unless drop_last is set.  With
+`max_annotations=Gcap` the example images fix a capacity of Bcap images of H x W, and the graph is captured on a static
+[Bcap, Gcap, 5] annotation table plus its device-side counts (models/losses.py).  Every call then takes images
+[B, 3, H, W] with 1 <= B <= Bcap and annotations [B, G, 5] with G <= Gcap, from the host or the device: the images go
+to the first B rows of the static input and the rest is zero-filled; one launch packs the annotations (each image's
+labelled rows first, the rest -1) and writes the counts; then the graph replays.  The loss is the mean over the B real
+images; the padding images are excluded from it and their gradients are exactly zero, and the frozen BatchNorm and the
+per-image squeeze-excite keep them from touching the real images.  A short batch costs a full-capacity step.  Images
+with more than Gcap annotations, more than Bcap images or another H x W are refused before anything is launched.
+
+    step = GraphedTrainStep(model, images_example, annotations_example, optimizer=opt, max_annotations=256)
+    for idx, (images, annotations) in enumerate(train_loader):       # any batch size up to Bcap, ragged annotations
+        loss = step(images, annotations, update=(idx + 1) % k == 0)
 
 Training with the optimizer in the graph.  With `optimizer=FusedClipAdamW(...)` every call is one micro-step of the
 reference loop (train.py:95-133): forward, loss, backward, gradients added to the persistent accumulators that
@@ -65,7 +79,7 @@ class GraphedTrainStep:
     init_process_group, the DDP wrapper CONSTRUCTED inside a side-stream context, >= 11 eager warm-up iterations);
     gradients then have to flow through DDP's AccumulateGrad hooks, so the captured step calls loss.backward()."""
 
-    def __init__(self, model, images, annotations, optimizer=None, warmup=3):
+    def __init__(self, model, images, annotations, optimizer=None, warmup=3, max_annotations=None):
         if not images.is_cuda:
             raise _ops.N.EffdetNativeError('GraphedTrainStep needs CUDA example inputs')
         self.ddp = isinstance(model, torch.nn.parallel.DistributedDataParallel)
@@ -75,7 +89,21 @@ class GraphedTrainStep:
         self.optimizer = optimizer
         self.fused = isinstance(optimizer, FusedClipAdamW)
         self.static_images = images.clone()
-        self.static_annots = annotations.clone()
+        self.static_counts = None
+        if max_annotations is None:
+            self.static_annots = annotations.clone()
+        else:
+            if isinstance(max_annotations, bool) or not isinstance(max_annotations, int) or max_annotations < 1:
+                raise _ops.N.EffdetNativeError('GraphedTrainStep: max_annotations must be an integer >= 1, got %r'
+                                               % (max_annotations,))
+            if images.dim() != 4:
+                raise _ops.N.EffdetNativeError('GraphedTrainStep: example images must be [Bcap, 3, H, W], got %s'
+                                               % (tuple(images.shape),))
+            self.static_annots = torch.full((images.shape[0], max_annotations, 5), -1.0, dtype=torch.float32,
+                                            device=images.device)
+            self.static_counts = torch.zeros((1 + images.shape[0],), dtype=torch.int32, device=images.device)
+            self._check_batch(images, annotations)
+            self._load_batch(images, annotations)
         params = [p for p in model.parameters() if p.requires_grad]
         side = torch.cuda.Stream(device=images.device)
         side.wait_stream(torch.cuda.current_stream(images.device))
@@ -114,7 +142,10 @@ class GraphedTrainStep:
         if zero:
             for p in params:
                 p.grad = None
-        cl, rl = self.model([self.static_images, self.static_annots])
+        inputs = [self.static_images, self.static_annots]
+        if self.static_counts is not None:
+            inputs.append(self.static_counts)
+        cl, rl = self.model(inputs)
         loss = cl.mean() + rl.mean()
         # torch.autograd.grad, not .backward(): AccumulateGrad nodes remember the stream of an earlier eager step (the
         # legacy stream if the caller still holds that step's loss) and would make it wait on the capturing stream --
@@ -132,9 +163,42 @@ class GraphedTrainStep:
             self.optimizer.step()
         return loss.detach()
 
+    def _check_batch(self, images, annotations):
+        """capacity mode: refuse a batch that does not fit, before anything is launched"""
+        cap = tuple(self.static_images.shape)
+        Bcap, Gcap = cap[0], self.static_annots.shape[1]
+        if images.dim() != 4 or tuple(images.shape[1:]) != cap[1:]:
+            raise _ops.N.EffdetNativeError('GraphedTrainStep was captured for images [B <= %d, %d, %d, %d], got %s'
+                                           % (cap + (tuple(images.shape),)))
+        B = images.shape[0]
+        if not 1 <= B <= Bcap:
+            raise _ops.N.EffdetNativeError('GraphedTrainStep: a batch of %d images does not fit the capacity of %d '
+                                           'images of the example' % (B, Bcap))
+        if annotations.dim() != 3 or annotations.shape[0] != B or annotations.shape[2] != 5:
+            raise _ops.N.EffdetNativeError('GraphedTrainStep: annotations must be [B=%d, G, 5], got %s'
+                                           % (B, tuple(annotations.shape)))
+        G = annotations.shape[1]
+        if G > Gcap:
+            raise _ops.N.EffdetNativeError('GraphedTrainStep: a batch with %d annotation rows per image does not fit '
+                                           'max_annotations=%d; build the step with max_annotations=%d or more'
+                                           % (G, Gcap, G))
+
+    def _load_batch(self, images, annotations):
+        """capacity mode: images into the static input (zeros after them), annotations packed with their counts"""
+        B = images.shape[0]
+        self.static_images[:B].copy_(images, non_blocking=True)
+        if B < self.static_images.shape[0]:
+            self.static_images[B:].zero_()
+        if annotations.shape[1] == 0:                                # no rows at all: one -1 row, as collater writes
+            annotations = torch.full((B, 1, 5), -1.0)
+        annotations = annotations.to(device=self.static_annots.device, dtype=torch.float32, non_blocking=True)
+        _ops.pack_annotations(annotations.contiguous(), self.static_annots, self.static_counts)
+
     def __call__(self, images, annotations, update=True):
         """One micro-step.  update: run the optimizer after it (train.py:115 `(idx + 1) % k == 0`); with
         FusedClipAdamW the update is skipped on the device when the step's loss is exactly zero."""
+        if self.static_counts is not None:
+            self._check_batch(images, annotations)
         if self.fused:
             if self.ddp and not update:
                 raise _ops.N.EffdetNativeError('GraphedTrainStep: update=False (gradient accumulation) is not supported '
@@ -143,8 +207,11 @@ class GraphedTrainStep:
         elif not update:
             raise _ops.N.EffdetNativeError('GraphedTrainStep: update=False (gradient accumulation) needs '
                                            'optimizer=FusedClipAdamW(...)')
-        self.static_images.copy_(images, non_blocking=True)
-        self.static_annots.copy_(annotations, non_blocking=True)
+        if self.static_counts is not None:
+            self._load_batch(images, annotations)
+        else:
+            self.static_images.copy_(images, non_blocking=True)
+            self.static_annots.copy_(annotations, non_blocking=True)
         self.graph.replay()
         return self.static_loss
 

@@ -5,6 +5,13 @@ returns ``(cls_loss[1], reg_loss[1])`` exactly like the reference (:152); IoU as
 "no annotation -> zero" branch (:54-58), ignore band 0.4..0.5 (:71-84), alpha/gamma = 0.25/2
 (:33-34), box targets with the 0.1/0.2 scaling (:116-136) and smooth-L1 beta 1/9 (:140-146) all run on
 the device with no host synchronisation and no per-image Python loop.
+
+Any number of annotation rows per image works.  Up to 256 rows the table is staged in shared memory whole; wider
+tables are staged in chunks of 256 rows, keeping each anchor's first maximum across the chunks.  The optional
+``counts`` ([1 + B] int32 on the device, as ``_ops.pack_annotations`` writes it) names the real images and each
+image's annotation rows without a host read: ``counts[0]`` images take part and the losses are their mean, image b
+reads only its first ``counts[1 + b]`` rows, and every image past ``counts[0]`` is padding, with no loss and exactly
+zero gradients.  That is how ``GraphedTrainStep(max_annotations=...)`` replays short and ragged batches in one graph.
 """
 import torch
 import torch.nn as nn
@@ -26,5 +33,5 @@ class FocalLoss(nn.Module):
     alpha = 0.25
     gamma = 2.0
 
-    def forward(self, classifications, regressions, anchors, annotations):
-        return _ops.FocalLossFn.apply(classifications, regressions, anchors, annotations, self.alpha, self.gamma)
+    def forward(self, classifications, regressions, anchors, annotations, counts=None):
+        return _ops.FocalLossFn.apply(classifications, regressions, anchors, annotations, self.alpha, self.gamma, counts)

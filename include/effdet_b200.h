@@ -326,6 +326,25 @@ int effdet_focal_loss_bwd(const float* cls, const float* reg, const float* ancho
                           const float* gout, const int32_t* assign_ws, const float* stats_ws, float* dcls,
                           float* dreg, int B, int A, int K, int G, float alpha, float gamma, int device,
                           effdet_stream_t stream);
+/* The same loss with the image and annotation counts in DEVICE memory, for any G >= 1 (the table is staged in
+ * chunks of 256 rows; an anchor's first maximum holds across chunks).
+ *   counts [1+B] int32: counts[0] = n_img (1..B), counts[1+b] = rows of image b that are read (0..G); values outside
+ *          those ranges are clamped.  Rows at or past counts[1+b] are never read, rows labelled -1 before it are skipped.
+ *   Images b >= n_img read nothing of cls, reg or annots: assign_ws -3, zero stats, dcls and dreg exactly 0.
+ *   losses and gradient scales average over n_img instead of B: gout[0] / (max(npos,1) * n_img), gout[1] / (4 npos n_img).
+ *   Refused before any launch: null pointers, B outside 1..65535, G < 1 (or G * 5 beyond int). */
+int effdet_focal_loss_counted_fwd(const float* cls, const float* reg, const float* anchors, const float* annots,
+                                  const int32_t* counts, float* losses, int32_t* assign_ws, float* stats_ws, int B, int A,
+                                  int K, int G, float alpha, float gamma, int device, effdet_stream_t stream);
+int effdet_focal_loss_counted_bwd(const float* cls, const float* reg, const float* anchors, const float* annots,
+                                  const int32_t* counts, const float* gout, const int32_t* assign_ws, const float* stats_ws,
+                                  float* dcls, float* dreg, int B, int A, int K, int G, float alpha, float gamma, int device,
+                                  effdet_stream_t stream);
+/* A ragged collated batch annots [B,G,5] (-1 padded) into a static table out [Bcap,Gcap,5] and its counts [1+Bcap]:
+ * per image the rows whose label is not -1, in their order, then -1 rows; counts[1+b] = rows kept (0 for b >= B),
+ * counts[0] = B.  No host read.  Refused before the launch: B outside 1..Bcap, G outside 1..Gcap, Bcap > 65535. */
+int effdet_pack_annots(const float* annots, int B, int G, float* out, int32_t* counts, int Bcap, int Gcap, int device,
+                       effdet_stream_t stream);
 /* y = g * p*(1-p) (sigmoid backward) ; y may alias g */
 int effdet_sigmoid_bwd(const float* g, const float* p, float* y, int64_t n, int device, effdet_stream_t stream);
 /* ------------------------------------------------------------------------------------------
