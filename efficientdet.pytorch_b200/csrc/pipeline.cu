@@ -120,6 +120,100 @@ __global__ void __launch_bounds__(256) resize_normalize_pad_kernel(const uint8_t
     o[2 * plane] = (float)v[2];
 }
 
+// demo.py's test transform, get_augumentation(phase='test') (datasets/augmentation.py:38-48, albumentations 0.5.2):
+// Resize(H, W) = cv2.resize(frame, (W, H), INTER_LINEAR) on the uint8 BGR frame, then Normalize and ToTensor in float32.
+// Unlike Resizer's float64 resize above, OpenCV resizes CV_8U in fixed point (tools/frame_oracle.py states the rules):
+//   same size            : copy
+//   src/dst == 2 on both : INTER_AREA's 2x2 box, (S00 + S01 + S10 + S11 + 2) >> 2
+//   otherwise            : per axis f = float((d + 0.5) * (1 / (dst / src)) - 0.5), s = floor(f), f -= s (float32);
+//                          columns clamp s < 0 to (0, 0) and s >= w - 1 to (w - 1, 0), second tap clamped to w - 1;
+//                          rows keep f and clamp both row indices into [0, h - 1].  Taps a = rint((1 - f) * 2048),
+//                          rint(f * 2048); H(r) = S[r][s] * a0 + S[r][s + 1] * a1 (int32, scale 2^11);
+//                          out = ((((H(r0) >> 4) * b0) >> 16) + (((H(r1) >> 4) * b1) >> 16) + 2) >> 2, OpenCV's vector
+//                          rounding (the scalar (H0 * b0 + H1 * b1 + 2^21) >> 22 differs in about a third of the pixels).
+// Normalize: mean * 255 and std * 255 in float32, den = 1 / (std * 255) rounded once, then (float(u8) - mean) * den, each
+// step rounded on its own (no FMA).  The channels keep the frame's byte order (BGR from cv2.imread).
+// One thread per output pixel (x fastest), at most 4 source pixels each; a frame with h == 0 is padding and writes zeros.
+__global__ void __launch_bounds__(256) frame_transform_kernel(const uint8_t* __restrict__ pix, const int64_t* __restrict__ offs,
+                                                              const int32_t* __restrict__ hw, float* __restrict__ out, int H,
+                                                              int W, float m0, float m1, float m2, float s0, float s1,
+                                                              float s2) {
+    const int b = blockIdx.z;
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const int y = blockIdx.y;
+    if (x >= W) return;
+    const int h = hw[2 * b], w = hw[2 * b + 1];
+    const long long plane = (long long)H * W;
+    float* o = out + (long long)b * 3 * plane + (long long)y * W + x;
+    if (h <= 0 || w <= 0) {
+        o[0] = o[plane] = o[2 * plane] = 0.f;
+        return;
+    }
+    const uint8_t* img = pix + offs[b];
+    auto px = [&](int r, int c) { return img + ((long long)r * w + c) * 3; };
+    int v[3];
+    const double scale_x = __ddiv_rn(1.0, __ddiv_rn((double)W, (double)w));
+    const double scale_y = __ddiv_rn(1.0, __ddiv_rn((double)H, (double)h));
+    if (h == H && w == W) {
+        const uint8_t* p = px(y, x);
+        for (int c = 0; c < 3; ++c) v[c] = p[c];
+    } else if (fabs(__dsub_rn(scale_x, 2.0)) < DBL_EPSILON && fabs(__dsub_rn(scale_y, 2.0)) < DBL_EPSILON) {
+        const uint8_t *p00 = px(2 * y, 2 * x), *p01 = px(2 * y, 2 * x + 1);
+        const uint8_t *p10 = px(2 * y + 1, 2 * x), *p11 = px(2 * y + 1, 2 * x + 1);
+        for (int c = 0; c < 3; ++c) v[c] = (p00[c] + p01[c] + p10[c] + p11[c] + 2) >> 2;
+    } else {
+        float fx = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)x, 0.5), scale_x), 0.5));
+        int sx = (int)floorf(fx);
+        fx = __fsub_rn(fx, (float)sx);
+        if (sx < 0) fx = 0.f, sx = 0;
+        if (sx >= w - 1) fx = 0.f, sx = w - 1;
+        const int sx1 = min(sx + 1, w - 1);
+        float fy = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)y, 0.5), scale_y), 0.5));
+        const int sy = (int)floorf(fy);
+        fy = __fsub_rn(fy, (float)sy);
+        const int r0 = min(max(sy, 0), h - 1), r1 = min(max(sy + 1, 0), h - 1);
+        const int a0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, fx), 2048.f)), a1 = __float2int_rn(__fmul_rn(fx, 2048.f));
+        const int b0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, fy), 2048.f)), b1 = __float2int_rn(__fmul_rn(fy, 2048.f));
+        const uint8_t *q00 = px(r0, sx), *q01 = px(r0, sx1), *q10 = px(r1, sx), *q11 = px(r1, sx1);
+        for (int c = 0; c < 3; ++c) {
+            const int h0 = q00[c] * a0 + q01[c] * a1, h1 = q10[c] * a0 + q11[c] * a1;
+            v[c] = min(max((((h0 >> 4) * b0 >> 16) + ((h1 >> 4) * b1 >> 16) + 2) >> 2, 0), 255);
+        }
+    }
+    const float mean[3] = {__fmul_rn(m0, 255.f), __fmul_rn(m1, 255.f), __fmul_rn(m2, 255.f)};
+    const float den[3] = {__frcp_rn(__fmul_rn(s0, 255.f)), __frcp_rn(__fmul_rn(s1, 255.f)), __frcp_rn(__fmul_rn(s2, 255.f))};
+    for (int c = 0; c < 3; ++c) o[c * plane] = __fmul_rn(__fsub_rn((float)v[c], mean[c]), den[c]);
+}
+
+// demo.py:86-104 on the padded detections of a batch of frames: per kept row of frame b (h x w), in network-input
+// pixels of an H x W input,
+//   x = int(bbox[0] * w / W) (and y1, x2, y2 likewise), float32 product and quotient (NumPy >= 2, NEP 50), truncated;
+//   score = int(np.around(s, 2) * 100) = trunc(rint(s * 100) / 100 * 100) in float32, rint half to even;
+//   label = the row's class.
+// rows [B, C, 6] int32 (x1, y1, x2, y2, label, score): rows past out_count[b] are not written.  out_count[b] = count[b],
+// 0 for a padding frame (h == 0), -1 when the frame overflowed the candidate cap.  Grid (C / 256, B).
+__global__ void __launch_bounds__(256) frame_boxes_kernel(const float* __restrict__ scores, const int64_t* __restrict__ classes,
+                                                          const float4* __restrict__ boxes, const int32_t* __restrict__ count,
+                                                          const int32_t* __restrict__ hw, int32_t* __restrict__ rows,
+                                                          int32_t* __restrict__ out_count, int C, float H, float W) {
+    const int b = blockIdx.y;
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    const int h = hw[2 * b], w = hw[2 * b + 1];
+    const int n = h > 0 ? count[b] : 0;
+    if (k == 0) out_count[b] = n;
+    if (k >= n || k >= C) return;
+    const long long i = (long long)b * C + k;
+    const float4 bx = boxes[i];
+    const float fw = (float)w, fh = (float)h;
+    int32_t* r = rows + i * 6;
+    r[0] = (int)__fdiv_rn(__fmul_rn(bx.x, fw), W);
+    r[1] = (int)__fdiv_rn(__fmul_rn(bx.y, fh), H);
+    r[2] = (int)__fdiv_rn(__fmul_rn(bx.z, fw), W);
+    r[3] = (int)__fdiv_rn(__fmul_rn(bx.w, fh), H);
+    r[4] = (int)classes[i];
+    r[5] = (int)__fmul_rn(__fdiv_rn(rintf(__fmul_rn(scores[i], 100.f)), 100.f), 100.f);
+}
+
 // annotations: rows [n_b, 5] float64 (x1, y1, x2, y2, label) concatenated over the batch -> float32 [B, G, 5], -1 padded.
 // Resizer scales the box by `scale` (float64), Augmenter mirrors x about the image width BEFORE the resize.
 __global__ void collate_annots_kernel(const double* __restrict__ rows, const int32_t* __restrict__ row_off,
@@ -180,6 +274,33 @@ extern "C" int effdet_resize_normalize_pad(const uint8_t* pixels, const int64_t*
                                                                        pixel_scale == 255, mean3[0], mean3[1], mean3[2],
                                                                        std3[0], std3[1], std3[2]);
     return launch_status("resize_normalize_pad_kernel");
+}
+
+extern "C" int effdet_frame_transform(const uint8_t* pixels, const int64_t* offsets, const int32_t* hw, float* out_nchw, int B,
+                                      int H, int W, const float* mean3, const float* std3, int device, effdet_stream_t stream) {
+    EFFDET_REQUIRE(pixels && offsets && hw && out_nchw && mean3 && std3, "frame_transform: null argument");
+    EFFDET_REQUIRE(B >= 1 && B <= 65535, "frame_transform: B=%d must be in [1, 65535]", B);
+    EFFDET_REQUIRE(H >= 1 && H <= 65535 && W >= 1 && W <= 65535, "frame_transform: H=%d, W=%d must be in [1, 65535]", H, W);
+    EFFDET_DEVICE(device);
+    dim3 grid(cdiv(W, 256), H, B);
+    frame_transform_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(pixels, offsets, hw, out_nchw, H, W, mean3[0], mean3[1],
+                                                                  mean3[2], std3[0], std3[1], std3[2]);
+    return launch_status("frame_transform_kernel");
+}
+
+extern "C" int effdet_frame_boxes(const float* scores, const int64_t* classes, const float* boxes, const int32_t* count,
+                                  const int32_t* hw, int B, int C, int H, int W, int32_t* rows, int32_t* out_count, int device,
+                                  effdet_stream_t stream) {
+    EFFDET_REQUIRE(scores && classes && boxes && count && hw && rows && out_count, "frame_boxes: null argument");
+    EFFDET_REQUIRE(B >= 1 && B <= 65535, "frame_boxes: B=%d must be in [1, 65535]", B);
+    EFFDET_REQUIRE(C >= 1, "frame_boxes: C=%d must be >= 1", C);
+    EFFDET_REQUIRE(H >= 1 && W >= 1, "frame_boxes: H=%d, W=%d must be >= 1", H, W);
+    EFFDET_REQUIRE(aligned16(boxes), "frame_boxes: boxes must be 16-byte aligned");
+    EFFDET_DEVICE(device);
+    dim3 grid(cdiv(C, 256), B);
+    frame_boxes_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scores, classes, reinterpret_cast<const float4*>(boxes), count,
+                                                              hw, rows, out_count, C, (float)H, (float)W);
+    return launch_status("frame_boxes_kernel");
 }
 
 extern "C" int effdet_collate_annots(const double* rows, const int32_t* row_off, const double* scale, const uint8_t* flip,

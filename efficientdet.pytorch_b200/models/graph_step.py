@@ -1,5 +1,5 @@
 """CUDA-graph execution of the training step (forward + FocalLoss + backward, optionally the fused optimizer), and of
-inference (GraphedDetect, at the end of this file).
+inference (GraphedDetect, and GraphedFrameDetect for demo.py's frames, at the end of this file).
 
 Every kernel of the hot path is launched on the caller's stream with device-resident arguments and no host
 synchronisation (the C ABI never syncs, FocalLoss reads its upstream gradients from device memory), so the ~480
@@ -67,9 +67,11 @@ With an optimizer in the graph the packed-weight / folded-BN derivations are cap
 replay because the weights change without Python seeing it.  For the same reason, eager use of the model between
 replays needs `model.eval()` / `model.train()` (or `_ops.invalidate_caches()`) first.
 """
+import numpy as np
 import torch
 
 from . import _ops
+from . import pipeline
 from .fused_optim import FusedClipAdamW
 
 
@@ -273,11 +275,15 @@ class GraphedDetect:
                                 self.threshold, self.iou_threshold, cap=_ops.candidate_cap(self.max_candidates, cls))
         return cls, reg, anchors, out
 
-    def __call__(self, images):
+    def _check_thresholds(self):
         if (self.model.threshold, self.model.iou_threshold) != (self.threshold, self.iou_threshold):
             raise _ops.N.EffdetNativeError(
-                'GraphedDetect: threshold / iou_threshold changed from (%r, %r) at capture to (%r, %r); build a new '
-                'GraphedDetect' % (self.threshold, self.iou_threshold, self.model.threshold, self.model.iou_threshold))
+                '%s: threshold / iou_threshold changed from (%r, %r) at capture to (%r, %r); build a new %s'
+                % (type(self).__name__, self.threshold, self.iou_threshold, self.model.threshold,
+                   self.model.iou_threshold, type(self).__name__))
+
+    def __call__(self, images):
+        self._check_thresholds()
         if images.shape != self.static_images.shape:
             raise _ops.N.EffdetNativeError('GraphedDetect was captured for images of shape %s, got %s'
                                            % (tuple(self.static_images.shape), tuple(images.shape)))
@@ -296,3 +302,91 @@ class GraphedDetect:
             else:
                 res.append([out.scores[b, :m], out.classes[b, :m], out.boxes[b, :m]])
         return res
+
+
+class GraphedFrameDetect(GraphedDetect):
+    """demo.py's Detect.process (demo.py:71-104) for a batch of frames as one CUDA-graph replay: the test transform
+    (pipeline.frame_transform's kernel) at the head of GraphedDetect's captured region, decode + NMS after the network,
+    and demo.py's per-box arithmetic (pipeline.frame_boxes) at its tail.
+
+        det = GraphedFrameDetect(model, example_frames)           # model.eval(), model.is_training False
+        for boxes, labels, scores in det(frames):                 # frames: list of uint8 [h, w, 3] BGR arrays
+            ...  # boxes int32 [n, 4], labels int64 [n], scores int32 [n]: demo.py's bboxes, label indices, bbox_scores
+
+    The example frames fix the capacity: Bcap = len(example_frames) frames and their total byte count.  A call takes
+    1 .. Bcap frames of any sizes whose bytes fit; it copies them and their geometry into pinned staging, issues the
+    host-to-device copies, replays once and reads back the counts and the kept rows (two device->host reads, no
+    per-box Python).  Frames of new sizes replay without recapture; unused capacity runs as zero padding frames.  A
+    frame that overflows max_candidates (None: every anchor may be a candidate, no frame overflows) is redone eagerly
+    from the replay's network outputs.  The network input is height x width, demo.py's size_image."""
+
+    def __init__(self, model, example_frames, height=512, width=512, max_candidates=None, warmup=2):
+        frames = pipeline.check_frames(example_frames, 'GraphedFrameDetect')
+        self.H, self.W = int(height), int(width)
+        if not (1 <= self.H <= 65535 and 1 <= self.W <= 65535):
+            raise _ops.N.EffdetNativeError('GraphedFrameDetect: height=%r, width=%r must be in [1, 65535]'
+                                           % (height, width))
+        dev = next(model.parameters()).device
+        if dev.type != 'cuda':
+            raise _ops.N.EffdetNativeError('GraphedFrameDetect needs a model on a CUDA device')
+        self.capacity = len(frames)
+        self.byte_capacity = sum(f.size for f in frames)
+        self._pix_h = torch.empty((self.byte_capacity,), dtype=torch.uint8).pin_memory()
+        self._offs_h = torch.zeros((self.capacity,), dtype=torch.int64).pin_memory()
+        self._hw_h = torch.zeros((self.capacity, 2), dtype=torch.int32).pin_memory()
+        self._pix = torch.empty((self.byte_capacity,), dtype=torch.uint8, device=dev)
+        self._offs = torch.empty((self.capacity,), dtype=torch.int64, device=dev)
+        self._hw = torch.empty((self.capacity, 2), dtype=torch.int32, device=dev)
+        self._load(frames)
+        super().__init__(model, torch.zeros((self.capacity, 3, self.H, self.W), device=dev), max_candidates, warmup)
+
+    def _load(self, frames):
+        """staging <- frames (padding frames h = w = 0 after them), then the host->device copies"""
+        B = len(frames)
+        flat, offs = pipeline.concat_pinned(frames, self._pix_h)
+        self._offs_h.zero_()
+        self._hw_h.zero_()
+        self._offs_h.numpy()[:B] = offs
+        self._hw_h.numpy()[:B] = [f.shape[:2] for f in frames]
+        self._pix[:flat.numel()].copy_(flat, non_blocking=True)
+        self._offs.copy_(self._offs_h, non_blocking=True)
+        self._hw.copy_(self._hw_h, non_blocking=True)
+
+    @torch.no_grad()
+    def _run(self):
+        pipeline.launch_frame_transform(self.static_images, self._pix, self._offs, self._hw)
+        cls, reg, anchors, out = super()._run()
+        self.rows, self.counts = pipeline.frame_boxes(out, self._hw, self.H, self.W)
+        return cls, reg, anchors, out
+
+    def __call__(self, frames):
+        """frames: list of 1 .. capacity uint8 [h, w, 3] arrays -> per frame (boxes int32 [n, 4], labels int64 [n],
+        scores int32 [n]) as NumPy arrays"""
+        frames = pipeline.check_frames(frames, 'GraphedFrameDetect')
+        B, nbytes = len(frames), sum(f.size for f in frames)
+        if B > self.capacity or nbytes > self.byte_capacity:
+            raise _ops.N.EffdetNativeError(
+                'GraphedFrameDetect: %d frames of %d bytes do not fit the capacity of %d frames and %d bytes of the '
+                'example frames' % (B, nbytes, self.capacity, self.byte_capacity))
+        self._check_thresholds()
+        self._load(frames)
+        self.graph.replay()
+        counts = self.counts[:B].tolist()                             # device->host read 1 of 2
+        top = max(counts + [0])
+        rows = self.rows[:B, :top].cpu().numpy() if top else None      # device->host read 2 of 2
+        res = []
+        for b, n in enumerate(counts):
+            if n < 0:
+                r = self._redo(b)
+            else:
+                r = rows[b, :n] if n else np.zeros((0, 6), np.int32)
+            res.append((np.ascontiguousarray(r[:, :4]), r[:, 4].astype(np.int64), np.ascontiguousarray(r[:, 5])))
+        return res
+
+    def _redo(self, b):
+        """rows of a frame that overflowed the candidate cap: eager NMS on the replay's network outputs"""
+        from .evaluation import _padded
+        trip = _ops.detect_batch(self.cls[b:b + 1], self.reg[b:b + 1], self.anchors, self.H, self.W, self.threshold,
+                                 self.iou_threshold)[0]
+        rows, counts = pipeline.frame_boxes(_padded(trip), self._hw[b:b + 1], self.H, self.W)
+        return rows[0, :int(counts[0])].cpu().numpy()

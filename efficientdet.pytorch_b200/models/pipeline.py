@@ -7,6 +7,10 @@
                       resize=True, to OpenCV's generic INTER_LINEAR resize).
   select_detections   eval.py:105-128 after NMS: boxes /= scale, score threshold, top-100, per-label split, without
                       the three .cpu().numpy() round trips per image.
+  frame_transform     demo.py's test transform (get_augumentation('test'): cv2.resize of the uint8 frame, Normalize,
+                      ToTensor) + unsqueeze / stack + .to(device), in one launch; frame_boxes is demo.py's per-box
+                      arithmetic on the padded detections.  GraphedFrameDetect (models/graph_step.py) runs both around
+                      the network in one CUDA graph.
 """
 import ctypes
 
@@ -26,6 +30,18 @@ def resizer_geometry(h, w, common_size):
         return scale, common_size, int(w * scale)
     scale = common_size / w
     return scale, int(h * scale), common_size
+
+
+def concat_pinned(imgs, staging=None):
+    """uint8 arrays back to back in pinned host memory -> (flat pinned uint8 tensor, int64 [B] byte offsets).
+    staging: a pinned uint8 tensor of at least the total size to write into, instead of a new allocation."""
+    nbytes = [im.size for im in imgs]
+    offs = np.concatenate([[0], np.cumsum(nbytes)[:-1]]).astype(np.int64)
+    if staging is None:
+        return torch.from_numpy(np.concatenate([im.reshape(-1) for im in imgs])).pin_memory(), offs
+    flat = staging[:sum(nbytes)]
+    np.concatenate([im.reshape(-1) for im in imgs], out=flat.numpy())
+    return flat, offs
 
 
 class DeviceCollater:
@@ -78,9 +94,7 @@ class DeviceCollater:
         else:
             scales = np.array([float(s.get('scale', 1.0)) for s in samples], dtype=np.float64)
             resized = sizes
-        nbytes = [im.size for im in imgs]
-        offs = np.concatenate([[0], np.cumsum(nbytes)[:-1]]).astype(np.int64)
-        flat = torch.from_numpy(np.concatenate([im.reshape(-1) for im in imgs])).pin_memory()
+        flat, offs = concat_pinned(imgs)
         flips = np.array([1 if s.get('flip') else 0 for s in samples], dtype=np.uint8)
         anns = [np.asarray(s['annot'], dtype=np.float64).reshape(-1, 5) for s in samples]
         counts = np.array([a.shape[0] for a in anns], dtype=np.int32)
@@ -123,3 +137,64 @@ def select_detections(scores, labels, boxes, scale, score_threshold=0.05, max_de
            int(num_classes), N.f32(dets), N.ptr(labs), N.ptr(offs), N.ptr(cnt))
     m = int(cnt.item())
     return dets[:m], labs[:m], offs
+
+
+def check_frames(frames, who):
+    """demo.py's frames as the device path takes them: a non-empty list of uint8 [h, w, 3] arrays with h, w >= 1
+    (cv2.imread's BGR layout) -> the same frames as C-contiguous arrays.  Raises before anything is copied."""
+    if isinstance(frames, np.ndarray) or not len(frames):
+        raise N.EffdetNativeError('%s: frames must be a non-empty list of uint8 [h, w, 3] arrays' % who)
+    out = []
+    for f in frames:
+        f = np.asarray(f)
+        if f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape[0] < 1 or f.shape[1] < 1:
+            raise N.EffdetNativeError('%s: frames must be uint8 [h, w, 3] with h, w >= 1, got %s %s'
+                                      % (who, f.dtype, f.shape))
+        out.append(np.ascontiguousarray(f))
+    if len(out) > 65535:
+        raise N.EffdetNativeError('%s: %d frames exceed 65535' % (who, len(out)))
+    return out
+
+
+_FRAME_MEAN = (ctypes.c_float * 3)(*MEAN)      # albumentations.Normalize's arguments, datasets/augmentation.py:44-45
+_FRAME_STD = (ctypes.c_float * 3)(*STD)
+
+
+def launch_frame_transform(out, pixels, offsets, hw):
+    """effdet_frame_transform of the frames in device memory (pixels uint8, offsets int64 [B], hw int32 [B, 2], h == 0
+    for padding) into out float32 [B, 3, H, W]"""
+    B, _, H, W = out.shape
+    N.call('effdet_frame_transform', out, N.ptr(pixels), N.ptr(offsets), N.ptr(hw), N.f32(out), B, H, W, _FRAME_MEAN,
+           _FRAME_STD, nbytes=float(pixels.numel() + 4 * out.numel()))
+
+
+def frame_transform(frames, height=512, width=512, device='cuda:0'):
+    """demo.py's `self.transform(image=img)['image'].to(device).unsqueeze(0)` (demo.py:75-78) for a list of uint8
+    [h, w, 3] BGR frames of any sizes -> float32 [B, 3, height, width] on `device`, bit-identical to albumentations
+    0.5.2's Resize (OpenCV's uint8 INTER_LINEAR) + Normalize + ToTensor, stacked.  Eager: one launch."""
+    frames = check_frames(frames, 'frame_transform')
+    if not (1 <= int(height) <= 65535 and 1 <= int(width) <= 65535):
+        raise N.EffdetNativeError('frame_transform: height=%r, width=%r must be in [1, 65535]' % (height, width))
+    dev = torch.device(device)
+    flat, offs = concat_pinned(frames)
+    sizes = np.array([f.shape[:2] for f in frames], dtype=np.int32)
+    d = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev, non_blocking=True)   # noqa: E731
+    out = torch.empty((len(frames), 3, int(height), int(width)), device=dev, dtype=torch.float32)
+    launch_frame_transform(out, flat.to(dev, non_blocking=True), d(offs), d(sizes))
+    return out
+
+
+def frame_boxes(detections, hw, height, width):
+    """demo.py:86-104 on padded detections (scores [B,C], classes [B,C] int64, boxes [B,C,4], count [B] int32, as
+    GraphedDetect returns them) of frames hw int32 [B, 2] on the device, for a network input of height x width
+    -> (rows int32 [B, C, 6] (x1, y1, x2, y2, label, score) valid below counts[b], counts int32 [B]: -1 for a frame that
+    overflowed the candidate cap, 0 for a padding frame).  No host read: capturable."""
+    scores, classes, boxes, count = detections
+    B, C = scores.shape
+    rows = torch.empty((B, C, 6), device=scores.device, dtype=torch.int32)
+    counts = torch.empty((B,), device=scores.device, dtype=torch.int32)
+    if classes.dtype != torch.int64 or count.dtype != torch.int32 or hw.dtype != torch.int32 or hw.numel() != 2 * B:
+        raise N.EffdetNativeError('frame_boxes: classes must be int64, count and hw int32 [B] / [B, 2]')
+    N.call('effdet_frame_boxes', scores, N.f32(scores, 'scores'), N.ptr(classes.contiguous()), N.f32(boxes, 'boxes'),
+           N.ptr(count.contiguous()), N.ptr(hw.contiguous()), B, C, int(height), int(width), N.ptr(rows), N.ptr(counts))
+    return rows, counts

@@ -450,6 +450,26 @@ int effdet_collate_annots(const double* rows, const int32_t* row_off, const doub
 int effdet_resize_normalize_pad(const uint8_t* pixels, const int64_t* offsets, const int32_t* hw, const int32_t* resized_hw,
                                 const uint8_t* flip, float* out_nchw, int B, int S, int pixel_scale, const double* mean3,
                                 const double* std3, int device, effdet_stream_t stream);
+/* demo.py's per-frame path (Detect.process, demo.py:71-104) for a batch of frames.
+ * effdet_frame_transform replaces get_augumentation(phase='test') + `.to(device).unsqueeze(0)` (demo.py:75-78,
+ * datasets/augmentation.py:38-48, albumentations 0.5.2): cv2.resize(frame, (W, H), INTER_LINEAR) of the uint8 frame in
+ * OpenCV's fixed-point CV_8U arithmetic, then Normalize ((float32(u8) - mean * 255) * float32(1 / (std * 255)), float32
+ * steps) and ToTensor, bit-identical to OpenCV 4.13.0 and NumPy.  Channels keep the frame's byte order (BGR).
+ *   pixels  : uint8 HWC frames back to back, frame b starts at byte offsets[b] and is hw[2b] x hw[2b+1] x 3 (any size
+ *             >= 1 x 1); hw[2b] == 0 marks a padding frame, whose output is zero
+ *   out_nchw: float32 [B,3,H,W];  mean3 / std3: 3 host floats (Normalize's mean and std, in [0, 1])
+ * effdet_frame_boxes replaces demo.py's per-box loop (demo.py:86-104) on the padded detections of the batch:
+ *   scores [B,C], classes [B,C] int64, boxes [B,C,4] (16-byte aligned), count [B] as GraphedDetect / detect_batch(cap=C)
+ *   write them; hw [2B] the frames' (h, w); H, W the network input's size (demo's size_image)
+ *   rows [B,C,6] int32: row k < out_count[b] of frame b is (int(x1 * w / W), int(y1 * h / H), int(x2 * w / W),
+ *        int(y2 * h / H), label, int(np.around(score, 2) * 100)), float32 arithmetic (NumPy >= 2); later rows are not
+ *        written.  out_count [B] int32: count[b], 0 for a padding frame, -1 when the frame overflowed the cap.
+ * Neither reads device memory on the host: both can be captured in a CUDA graph. */
+int effdet_frame_transform(const uint8_t* pixels, const int64_t* offsets, const int32_t* hw, float* out_nchw, int B, int H,
+                           int W, const float* mean3, const float* std3, int device, effdet_stream_t stream);
+int effdet_frame_boxes(const float* scores, const int64_t* classes, const float* boxes, const int32_t* count,
+                       const int32_t* hw, int B, int C, int H, int W, int32_t* rows, int32_t* out_count, int device,
+                       effdet_stream_t stream);
 /* SURVEY.md 8(f) rank 3: the step AFTER NMS (eval.py:105-128) for one image: boxes /= scale, score > threshold,
  * top-max_det by score (ties: lower input index), split per label.  out_dets [max_det,5] (x1,y1,x2,y2,score) grouped by
  * label ascending and in score order inside a label, out_labels [max_det], class_offsets [num_classes+1] (rows of label c
