@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.normpath(os.path.join(_HERE, '..', 'csrc'))
 SO_PATH = os.path.join(CSRC, 'libeffdet_b200.so')
 SOURCES = ['api.cu', 'conv_api.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_planes.cu', 'pw_gemm.cu', 'pw_wgrad.cu', 'stem.cu', 'dw_fused.cu', 'mbconv_ops.cu', 'se_ops.cu', 'bifpn.cu', 'pipeline.cu',
-           'loss.cu', 'detect.cu', 'layout.cu', 'optim.cu', 'voc_eval.cu', 'coco_eval.cu']
+           'loss.cu', 'detect.cu', 'soft_nms.cu', 'layout.cu', 'optim.cu', 'voc_eval.cu', 'coco_eval.cu']
 NVCC_FLAGS = ['-std=c++17', '-O3', '-lineinfo', '-gencode', 'arch=compute_90a,code=sm_90a',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -162,6 +162,7 @@ SIGNATURES = {
     'effdet_nms_batch': [_P, _P, _P, _INT, _INT, _INT, _INT, ctypes.c_double, _P, _P, _P] + _TAIL,
     'effdet_nms_batch_chunked': [_P, _P, _P] + [_INT] * 5 + [ctypes.c_double, _P, _I64, _P, _P] + _TAIL,
     'effdet_gather_detections_batch': [_P, _P, _P, _P, _P, _INT, _INT, _INT, _P, _P, _P] + _TAIL,
+    'effdet_soft_nms_batch': [_P] * 5 + [_INT] * 5 + [ctypes.c_double] * 2 + [_F, _P, _I64] + [_P] * 4 + _TAIL,
     'effdet_multi_sumsq': [_P, _P, _P, _P, _INT, _INT, _P] + _TAIL,
     'effdet_multi_clip_adamw': [_P] * 7 + [_INT, _INT, _P] + [_F] * 8 + [_INT] + _TAIL,
     'effdet_multi_accumulate': [_P] * 5 + [_INT, _INT] + [_P] * 3 + _TAIL,
@@ -186,7 +187,8 @@ PLAIN = {'effdet_version': (ctypes.c_int, []), 'effdet_conv_tc_kpad': (ctypes.c_
          'effdet_launch_count': (ctypes.c_uint64, []), 'effdet_reset_launch_count': (None, []),
          'effdet_voc_ap_workspace': (ctypes.c_int64, [ctypes.c_int] * 2),
          'effdet_coco_accumulate_workspace': (ctypes.c_int64, [ctypes.c_int] * 3),
-         'effdet_nms_chunked_workspace': (ctypes.c_int64, [ctypes.c_int] * 3)}
+         'effdet_nms_chunked_workspace': (ctypes.c_int64, [ctypes.c_int] * 3),
+         'effdet_soft_nms_workspace': (ctypes.c_int64, [ctypes.c_int] * 2)}
 
 _lib = None
 _lock = threading.Lock()

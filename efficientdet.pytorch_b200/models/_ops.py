@@ -8,6 +8,7 @@ Internal activation layout is NHWC fp32; module boundaries expose the same memor
 NCHW tensor with channels_last strides (zero-copy ``permute`` views).
 """
 import collections
+import math
 import os
 import weakref
 
@@ -1103,9 +1104,40 @@ def _nms_workspace(B, cap, chunk):
     return n
 
 
-def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=None):
+NMS_METHODS = {'hard': 0, 'linear': 1, 'gaussian': 2}          # 1, 2: EFFDET_SOFT_NMS_LINEAR / _GAUSSIAN
+
+
+def nms_method(nms, sigma, iou_threshold):
+    """the C code of post-processing method `nms` ('hard': greedy NMS, 'linear' / 'gaussian': Soft-NMS), after the
+    checks effdet_soft_nms_batch repeats: sigma finite and > 0, and for 'linear' iou_threshold in [0, 1]"""
+    if not isinstance(nms, str) or nms not in NMS_METHODS:
+        raise N.EffdetNativeError("nms=%r must be one of 'hard', 'linear', 'gaussian'" % (nms,))
+    try:
+        sigma = float(sigma)
+    except (TypeError, ValueError):
+        raise N.EffdetNativeError('soft_nms_sigma=%r must be a finite number > 0' % (sigma,)) from None
+    if not (math.isfinite(sigma) and sigma > 0):
+        raise N.EffdetNativeError('soft_nms_sigma=%r must be a finite number > 0' % (sigma,))
+    if nms == 'linear' and not 0.0 <= float(iou_threshold) <= 1.0:
+        raise N.EffdetNativeError("iou_threshold=%r must be in [0, 1] for nms='linear'" % (iou_threshold,))
+    return NMS_METHODS[nms]
+
+
+def _soft_nms_workspace(B, cap):
+    """bytes of effdet_soft_nms_batch's workspace, a multiple of 16 (0 up to cap = 32768)"""
+    n = int(N.load().effdet_soft_nms_workspace(B, cap))
+    if n < 0:
+        raise N.EffdetNativeError('detect_batch: %s' % N.last_error())
+    return n
+
+
+def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=None, nms='hard', sigma=0.5):
     """Decode + clip + class max + threshold + greedy NMS of every image of cls [B,A,K] / reg [B,A,4], one set of
     launches for the whole batch (the reference does this for image 0 only, models/efficientdet.py:73-86).
+
+    nms='hard' is torchvision's greedy NMS at iou_threshold.  nms='linear' / 'gaussian' is Soft-NMS
+    (effdet_soft_nms_batch): 'linear' decays by 1 - IoU above iou_threshold, 'gaussian' by exp(-IoU^2 / sigma); the
+    returned scores are the decayed ones, in pick order (non-increasing), all above threshold.
 
     cap=None: reads the B candidate counts once to set cap = their maximum and the B kept counts once to slice the
     results -> list of B triples [scores[K_b], classes[K_b] int64, boxes[K_b,4]] on the device (empty tensors when no
@@ -1113,6 +1145,7 @@ def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=
     cap=C: no host synchronisation, so the call can be captured in a CUDA graph -> Detections(scores [B,C],
     classes [B,C] int64, boxes [B,C,4], count [B] int32), rows past count[b] zero; count[b] == -1 when image b has
     more than C candidates (its rows are then all zero)."""
+    method = nms_method(nms, sigma, iou_threshold)
     check_cuda_f32(cls, 'classifications')
     check_cuda_f32(reg, 'regressions')
     cls, reg = _contig(cls), _contig(reg)
@@ -1134,23 +1167,37 @@ def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=
         if cap == 0:
             return [[cls.new_zeros(0), torch.zeros(0, dtype=torch.int64, device=dev), cls.new_zeros(0, 4)]
                     for _ in range(B)]
+    o_s = _empty((B, cap), cls)
+    o_c = torch.empty((B, cap), device=dev, dtype=torch.int64)
+    o_b = _empty((B, cap, 4), cls)
+    nkeep = torch.empty((B,), device=dev, dtype=torch.int32)
+    if method:
+        ws_bytes = _soft_nms_workspace(B, cap)
+        ws = torch.empty((max(ws_bytes, 16),), device=dev, dtype=torch.uint8)
+        N.call('effdet_soft_nms_batch', cls, N.f32(boxes), N.f32(scores), classes.data_ptr(), keys.data_ptr(),
+               count.data_ptr(), B, A, npad, cap, method, float(iou_threshold), float(sigma), float(threshold),
+               ws.data_ptr(), ws_bytes, N.f32(o_s), o_c.data_ptr(), N.f32(o_b), nkeep.data_ptr())
+    else:
+        _hard_nms(cls, boxes, scores, classes, keys, count, B, A, npad, cap, float(iou_threshold), o_s, o_c, o_b,
+                  nkeep)
+    if not eager:
+        return Detections(o_s, o_c, o_b, nkeep)
+    m = nkeep.tolist()                               # host read 2 of 2
+    return [[o_s[b, :m[b]], o_c[b, :m[b]], o_b[b, :m[b]]] for b in range(B)]
+
+
+def _hard_nms(cls, boxes, scores, classes, keys, count, B, A, npad, cap, iou_threshold, o_s, o_c, o_b, nkeep):
+    """greedy NMS (effdet_nms_batch_chunked) of the sorted candidates, then the gather into the padded outputs"""
+    dev = cls.device
     chunk = min(cap, NMS_CHUNK)
     per_image = _nms_workspace(1, cap, chunk)
     group = min(B, max(NMS_MASK_BUDGET, per_image) // per_image)
     ws_bytes = _nms_workspace(group, cap, chunk)
     ws = torch.empty((ws_bytes // 8,), device=dev, dtype=torch.int64)
     keep = torch.empty((B, cap), device=dev, dtype=torch.int32)
-    nkeep = torch.empty((B,), device=dev, dtype=torch.int32)
     for b0 in range(0, B, group):
         N.call('effdet_nms_batch_chunked', cls, N.f32(boxes[b0:]), keys[b0:].data_ptr(), count[b0:].data_ptr(),
-               min(group, B - b0), A, npad, cap, chunk, float(iou_threshold), ws.data_ptr(), ws_bytes,
+               min(group, B - b0), A, npad, cap, chunk, iou_threshold, ws.data_ptr(), ws_bytes,
                keep[b0:].data_ptr(), nkeep[b0:].data_ptr())
-    o_s = _empty((B, cap), cls)
-    o_c = torch.empty((B, cap), device=dev, dtype=torch.int64)
-    o_b = _empty((B, cap, 4), cls)
     N.call('effdet_gather_detections_batch', cls, N.f32(boxes), N.f32(scores), classes.data_ptr(), keep.data_ptr(),
            nkeep.data_ptr(), B, A, cap, N.f32(o_s), o_c.data_ptr(), N.f32(o_b))
-    if not eager:
-        return Detections(o_s, o_c, o_b, nkeep)
-    m = nkeep.tolist()                               # host read 2 of 2
-    return [[o_s[b, :m[b]], o_c[b, :m[b]], o_b[b, :m[b]]] for b in range(B)]

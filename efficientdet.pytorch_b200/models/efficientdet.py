@@ -6,6 +6,11 @@ around sm_90a kernels.  Same constructor, attributes, call convention and state-
            annotation rows each (models/losses.py); the rest of the batch is padding
   eval  :  model(image[1,3,H,W]) -> [scores[K], classes[K] int64, boxes[K,4]]            (reference :69-86)
 
+Post-processing follows the attributes threshold, iou_threshold, nms and soft_nms_sigma, which may be set after
+construction: nms='hard' (default) is the reference's torchvision NMS; 'linear' and 'gaussian' are Soft-NMS
+(Bodla et al., ICCV 2017), which decays the scores of overlapping boxes instead of dropping them and returns the
+decayed scores.
+
 What differs underneath: features stay NHWC end to end, the head writes the level-concatenated
 ``[B, sum(HWA), K]`` / ``[B, sum(HWA), 4]`` tensors directly (no ``torch.cat``), anchors are cached per input
 size, and decode + clip + threshold + NMS run on the device for the whole batch with two read-backs.
@@ -41,11 +46,13 @@ def _reference_reinit(model):
 
 class EfficientDet(nn.Module):
     def __init__(self, num_classes, network='efficientdet-d0', D_bifpn=3, W_bifpn=88, D_class=3, is_training=True,
-                 threshold=0.01, iou_threshold=0.5):
+                 threshold=0.01, iou_threshold=0.5, nms='hard', soft_nms_sigma=0.5):
         super().__init__()
         # D_class is accepted and ignored, as in the reference (the head depth is fixed at 4 convs)
         self.is_training = is_training
         self.threshold, self.iou_threshold = threshold, iou_threshold
+        self.nms, self.soft_nms_sigma = nms, soft_nms_sigma
+        self.postprocess()
         # registration order backbone -> neck -> bbox_head fixes the state-dict order
         self.backbone = EfficientNet.from_pretrained(MODEL_MAP[network])
         pyramid_channels = self.backbone.get_list_features()[-_PYRAMID_LEVELS:]
@@ -90,10 +97,18 @@ class EfficientDet(nn.Module):
         cls, reg, anchors = self._raw_predictions(images)
         return self.criterion(cls, reg, anchors, annotations, counts)
 
+    def postprocess(self):
+        """the post-processing settings as _ops.detect_batch's keyword arguments (threshold, iou_threshold, nms, sigma),
+        checked: an unknown nms, a soft_nms_sigma that is not finite and > 0, or a linear iou_threshold outside [0, 1]
+        raises EffdetNativeError"""
+        _ops.nms_method(self.nms, self.soft_nms_sigma, self.iou_threshold)
+        return dict(threshold=self.threshold, iou_threshold=self.iou_threshold, nms=self.nms,
+                    sigma=self.soft_nms_sigma)
+
     def _detections(self, image):
+        post = self.postprocess()
         cls, reg, anchors = self._raw_predictions(image)
-        found = _ops.detect_batch(cls[:1], reg[:1], anchors, image.shape[2], image.shape[3], self.threshold,
-                                  self.iou_threshold)[0]
+        found = _ops.detect_batch(cls[:1], reg[:1], anchors, image.shape[2], image.shape[3], **post)[0]
         if found[0].numel() == 0:
             print('No boxes to NMS')
             return [torch.zeros(0), torch.zeros(0), torch.zeros(0, 4)]
@@ -116,9 +131,9 @@ class EfficientDet(nn.Module):
         forward(images[i:i+1]).
         -> list of B triples [scores[K_i], classes[K_i] int64, boxes[K_i,4]] on the device (empty tensors when no
         anchor passes the threshold)."""
+        post = self.postprocess()
         cls, reg, anchors = self._raw_predictions(images)
-        return _ops.detect_batch(cls, reg, anchors, images.shape[2], images.shape[3], self.threshold,
-                                 self.iou_threshold)
+        return _ops.detect_batch(cls, reg, anchors, images.shape[2], images.shape[3], **post)
 
     def forward(self, inputs):
         if self.is_training:

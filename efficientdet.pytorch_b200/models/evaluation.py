@@ -130,8 +130,7 @@ def _add_batch(acc, out, cls, reg, anchors, hw, model, scales, *per_image):
             acc.add(_ops.Detections(*(t[b0:b] for t in out)), scales[b0:b], *(p[b0:b] for p in per_image))
         if m is None:
             break
-        trip = _ops.detect_batch(cls[b:b + 1], reg[b:b + 1], anchors, hw[0], hw[1], model.threshold,
-                                 model.iou_threshold)[0]
+        trip = _ops.detect_batch(cls[b:b + 1], reg[b:b + 1], anchors, hw[0], hw[1], **model.postprocess())[0]
         acc.add(_padded(trip), scales[b:b + 1], *(p[b:b + 1] for p in per_image))
         b0 = b + 1
 
@@ -156,8 +155,8 @@ def _detect_all(dataset, model, acc, batch_size, per_image, progress_base):
                 cls, reg, anchors = graphed.cls, graphed.reg, graphed.anchors
             else:
                 cls, reg, anchors = model._raw_predictions(images)
-                out = _ops.detect_batch(cls, reg, anchors, hw[0], hw[1], model.threshold, model.iou_threshold,
-                                        cap=_ops.candidate_cap(MAX_CANDIDATES, cls))
+                out = _ops.detect_batch(cls, reg, anchors, hw[0], hw[1], cap=_ops.candidate_cap(MAX_CANDIDATES, cls),
+                                        **model.postprocess())
             _add_batch(acc, out, cls, reg, anchors, hw, model, [d['scale'] for d in data], *per_image(idx))
             for i in idx:
                 print('{}/{}'.format(i + progress_base, n), end='\r')

@@ -238,7 +238,8 @@ class GraphedDetect:
     decoded anchors and their sort keys (24 bytes per anchor plus 8 per power-of-two padded anchor) do not depend on C.
 
     The packed weights and folded BatchNorm are derived inside the graph, so replays follow in-place weight updates
-    (load_state_dict, EMA copies).  The score and IoU thresholds are fixed at capture."""
+    (load_state_dict, EMA copies).  The post-processing settings (threshold, iou_threshold, nms, soft_nms_sigma) are
+    fixed at capture: changing one on the model makes the next call raise."""
 
     def __init__(self, model, images, max_candidates=8192, warmup=2):
         if model.training or model.is_training:
@@ -248,7 +249,7 @@ class GraphedDetect:
             raise _ops.N.EffdetNativeError('GraphedDetect needs CUDA example images')
         self.model = model
         self.max_candidates = None if max_candidates is None else int(max_candidates)
-        self.threshold, self.iou_threshold = model.threshold, model.iou_threshold
+        self.post = model.postprocess()
         self.static_images = images.clone()
         dev = images.device
         side = torch.cuda.Stream(device=dev)
@@ -272,15 +273,14 @@ class GraphedDetect:
     def _run(self):
         cls, reg, anchors = self.model._raw_predictions(self.static_images)
         out = _ops.detect_batch(cls, reg, anchors, self.static_images.shape[2], self.static_images.shape[3],
-                                self.threshold, self.iou_threshold, cap=_ops.candidate_cap(self.max_candidates, cls))
+                                cap=_ops.candidate_cap(self.max_candidates, cls), **self.post)
         return cls, reg, anchors, out
 
     def _check_thresholds(self):
-        if (self.model.threshold, self.model.iou_threshold) != (self.threshold, self.iou_threshold):
-            raise _ops.N.EffdetNativeError(
-                '%s: threshold / iou_threshold changed from (%r, %r) at capture to (%r, %r); build a new %s'
-                % (type(self).__name__, self.threshold, self.iou_threshold, self.model.threshold,
-                   self.model.iou_threshold, type(self).__name__))
+        now = self.model.postprocess()
+        if now != self.post:
+            raise _ops.N.EffdetNativeError('%s: the post-processing settings changed from %r at capture to %r; build a '
+                                           'new %s' % (type(self).__name__, self.post, now, type(self).__name__))
 
     def __call__(self, images):
         self._check_thresholds()
@@ -297,8 +297,7 @@ class GraphedDetect:
         for b, m in enumerate(out.count.tolist()):                   # the one device->host read
             if m < 0:
                 res.append(_ops.detect_batch(self.cls[b:b + 1], self.reg[b:b + 1], self.anchors,
-                                             self.static_images.shape[2], self.static_images.shape[3], self.threshold,
-                                             self.iou_threshold)[0])
+                                             self.static_images.shape[2], self.static_images.shape[3], **self.post)[0])
             else:
                 res.append([out.scores[b, :m], out.classes[b, :m], out.boxes[b, :m]])
         return res
@@ -386,7 +385,6 @@ class GraphedFrameDetect(GraphedDetect):
     def _redo(self, b):
         """rows of a frame that overflowed the candidate cap: eager NMS on the replay's network outputs"""
         from .evaluation import _padded
-        trip = _ops.detect_batch(self.cls[b:b + 1], self.reg[b:b + 1], self.anchors, self.H, self.W, self.threshold,
-                                 self.iou_threshold)[0]
+        trip = _ops.detect_batch(self.cls[b:b + 1], self.reg[b:b + 1], self.anchors, self.H, self.W, **self.post)[0]
         rows, counts = pipeline.frame_boxes(_padded(trip), self._hw[b:b + 1], self.H, self.W)
         return rows[0, :int(counts[0])].cpu().numpy()

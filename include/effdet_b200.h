@@ -386,6 +386,30 @@ int effdet_nms_batch_chunked(const float* boxes, const uint64_t* keys, const int
 int effdet_gather_detections_batch(const float* boxes, const float* scores, const int32_t* classes,
                                    const int32_t* keep_idx, const int32_t* nkeep, int B, int A, int cap, float* out_scores,
                                    int64_t* out_classes, float* out_boxes, int device, effdet_stream_t stream);
+/* Soft-NMS (Bodla et al., ICCV 2017, Algorithm 1) of the same candidates, written directly as padded detections in
+ * effdet_gather_detections_batch's layout.  Each pick emits the live candidate with the highest current score (ties:
+ * lower anchor index) and rescales every other live score s by a weight of its IoU ov with the pick (fp32 IoU as the
+ * greedy NMS computes it; 0 when the intersection is 0):
+ *   EFFDET_SOFT_NMS_LINEAR  : w = (double)ov > iou_threshold ? 1 - ov : 1                  (iou_threshold in [0, 1])
+ *   EFFDET_SOFT_NMS_GAUSSIAN: w = (float)exp(-((double)ov * ov) / sigma), in fp64           (iou_threshold unused)
+ *   s = s * w in fp32; a candidate with !(s > threshold) leaves the live set.
+ * Row i of image b is its i-th pick: the score at the moment of the pick (non-increasing down the rows), the
+ * candidate's class and box.  Rows from out_count[b] on are zero; out_count[b] = -1 (all rows zero) when count[b] > cap.
+ *   boxes, scores, classes [B,A], keys [B,npad], count [B]: as effdet_detect_candidates_batch writes them
+ *   1 <= B <= 65535, 1 <= cap <= A, sigma finite and > 0 (checked for either method)
+ *   workspace: effdet_soft_nms_workspace(B, cap) bytes (B*cap*24 rounded up to a multiple of 16), 16-byte aligned;
+ *              0 bytes (null allowed) unless cap > 32768
+ *   threshold: candidates whose score is not above it are never picked (effdet_detect_candidates_batch leaves none)
+ *   out_scores [B][cap], out_classes [B][cap] int64, out_boxes [B][cap][4] (16-byte aligned), out_count [B] int32
+ * One launch whose grid depends on B and cap only (capturable); no host read. */
+#define EFFDET_SOFT_NMS_LINEAR 1
+#define EFFDET_SOFT_NMS_GAUSSIAN 2
+int64_t effdet_soft_nms_workspace(int B, int cap);
+int effdet_soft_nms_batch(const float* boxes, const float* scores, const int32_t* classes, const uint64_t* keys,
+                          const int32_t* count, int B, int A, int npad, int cap, int method, double iou_threshold,
+                          double sigma, float threshold, void* workspace, int64_t workspace_bytes, float* out_scores,
+                          int64_t* out_classes, float* out_boxes, int32_t* out_count, int device,
+                          effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) rank 1: the optimizer step that follows backward in the reference loop,
