@@ -8,7 +8,9 @@
 //   Normalizer computes (img.astype(float32) - mean[float64]) / std[float64] in float64 and train.py casts to float32 on
 //   the device; collater writes float64 annotations into a float32 tensor.
 #include <cfloat>
+#include <climits>
 
+#include "block_scan.cuh"
 #include "common.cuh"
 
 namespace effdet {
@@ -244,6 +246,64 @@ __global__ void collate_annots_kernel(const double* __restrict__ rows, const int
     o[4] = (float)r[4];
 }
 
+// collate_annots_kernel followed by pack_annots_kernel (loss.cu) in one pass, for the annotation sections of a raw batch
+// (models/pipeline.py RawBatch): B = header[0] images; image b owns rows row_off[b] .. row_off[b+1].  Each row is
+// flipped (fp64, before the scale), scaled by __dmul_rn and cast to float32 exactly as collate_annots_kernel does, then
+// kept unless its float32 label is -1, in order, into the front of slot b of out [Bcap,Gcap,5], -1 rows after them.
+// counts[1+b] = rows kept (0 for b >= B), counts[0] = B.  One CTA per slot b < Bcap; every image has <= Gcap rows (the
+// host checks it).
+__global__ void __launch_bounds__(256) collate_pack_annots_kernel(const int64_t* __restrict__ header,
+                                                                  const double* __restrict__ rows,
+                                                                  const int32_t* __restrict__ row_off,
+                                                                  const double* __restrict__ scale,
+                                                                  const uint8_t* __restrict__ flip,
+                                                                  const int32_t* __restrict__ hw, float* __restrict__ out,
+                                                                  int32_t* __restrict__ counts, int Gcap) {
+    __shared__ int warp_tot[32];
+    const int b = blockIdx.x;
+    const int B = (int)header[0];
+    float* dst = out + (long long)b * Gcap * 5;
+    int kept = 0;
+    if (b < B) {
+        const int r_begin = row_off[b], n = row_off[b + 1] - r_begin;
+        const bool fl = flip[b] != 0;
+        const double cols = (double)hw[2 * b + 1], sc = scale[b];
+        for (int g0 = 0; g0 < n; g0 += blockDim.x) {                    // CTA-uniform trip count
+            const int g = g0 + threadIdx.x;
+            float v[5];
+            bool keep = false;
+            if (g < n) {
+                const double* r = rows + (long long)(r_begin + g) * 5;
+                double x1 = r[0], x2 = r[2];
+                if (fl) {                                               // annots[:, 0] = cols - x2 ; annots[:, 2] = cols - x1
+                    const double nx1 = __dsub_rn(cols, x2), nx2 = __dsub_rn(cols, x1);
+                    x1 = nx1;
+                    x2 = nx2;
+                }
+                v[0] = (float)__dmul_rn(x1, sc);                        // annots[:, :4] *= scale, then the float32 table
+                v[1] = (float)__dmul_rn(r[1], sc);
+                v[2] = (float)__dmul_rn(x2, sc);
+                v[3] = (float)__dmul_rn(r[3], sc);
+                v[4] = (float)r[4];
+                keep = v[4] != -1.f;
+            }
+            int total;
+            const int incl = block_scan(keep ? 1 : 0, warp_tot, IntAdd(), total);
+            if (keep) {
+                float* o = dst + (long long)(kept + incl - 1) * 5;
+#pragma unroll
+                for (int c = 0; c < 5; ++c) o[c] = v[c];
+            }
+            kept += total;
+        }
+    }
+    for (long long i = (long long)kept * 5 + threadIdx.x; i < (long long)Gcap * 5; i += blockDim.x) dst[i] = -1.f;
+    if (threadIdx.x == 0) {
+        counts[1 + b] = kept;
+        if (b == 0) counts[0] = B;
+    }
+}
+
 }  // namespace effdet
 
 using namespace effdet;
@@ -309,4 +369,16 @@ extern "C" int effdet_collate_annots(const double* rows, const int32_t* row_off,
     EFFDET_DEVICE(device);
     collate_annots_kernel<<<cdiv((long long)B * G, 128), 128, 0, (cudaStream_t)stream>>>(rows, row_off, scale, flip, width, out, B, G);
     return launch_status("collate_annots_kernel");
+}
+
+extern "C" int effdet_collate_pack_annots(const int64_t* header, const double* rows, const int32_t* row_off,
+                                          const double* scale, const uint8_t* flip, const int32_t* hw, float* out,
+                                          int32_t* counts, int Bcap, int Gcap, int device, effdet_stream_t stream) {
+    EFFDET_REQUIRE(header && rows && row_off && scale && flip && hw && out && counts, "collate_pack_annots: null argument");
+    EFFDET_REQUIRE(Bcap > 0 && Bcap <= 65535 && Gcap > 0 && Gcap <= INT_MAX / 5,
+                   "collate_pack_annots: capacity Bcap=%d, Gcap=%d unsupported (1..65535, 1..%d)", Bcap, Gcap, INT_MAX / 5);
+    EFFDET_DEVICE(device);
+    collate_pack_annots_kernel<<<Bcap, 256, 0, (cudaStream_t)stream>>>(header, rows, row_off, scale, flip, hw, out, counts,
+                                                                      Gcap);
+    return launch_status("collate_pack_annots_kernel");
 }

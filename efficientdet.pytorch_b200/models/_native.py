@@ -170,6 +170,7 @@ SIGNATURES = {
     'effdet_normalize_pad': [_P, _P, _P, _P, _P, _INT, _INT, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)] + _TAIL,
     'effdet_resize_normalize_pad': [_P] * 6 + [_INT] * 3 + [ctypes.POINTER(ctypes.c_double)] * 2 + _TAIL,
     'effdet_collate_annots': [_P, _P, _P, _P, _P, _P, _INT, _INT] + _TAIL,
+    'effdet_collate_pack_annots': [_P] * 8 + [_INT, _INT] + _TAIL,
     'effdet_frame_transform': [_P] * 4 + [_INT] * 3 + [ctypes.POINTER(ctypes.c_float)] * 2 + _TAIL,
     'effdet_frame_boxes': [_P] * 5 + [_INT] * 4 + [_P, _P] + _TAIL,
     'effdet_eval_select': [_P, _P, _P, _INT, _F, _F, _INT, _INT, _P, _P, _P, _P] + _TAIL,

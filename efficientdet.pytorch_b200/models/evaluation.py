@@ -21,7 +21,8 @@ import torch
 
 from . import _native as N
 from . import _ops
-from .graph_step import GraphedDetect
+from . import pipeline
+from .graph_step import GraphedDetect, GraphedRawDetect
 
 # candidate rows per image that the graphed detection keeps before NMS: None = every anchor, so no image overflows; with
 # an integer, an image with more candidates is redone eagerly
@@ -135,10 +136,50 @@ def _add_batch(acc, out, cls, reg, anchors, hw, model, scales, *per_image):
         b0 = b + 1
 
 
-def _detect_all(dataset, model, acc, batch_size, per_image, progress_base):
+def _detect_raw(dataset, model, acc, batch_size, per_image, progress_base, collater, num_workers):
+    """_detect_all for a dataset of decoded samples: a DataLoader with collate_fn=collater (a RawCollater) yields raw
+    batches, full batches replay one GraphedRawDetect (the Resizer chain runs at the head of its graph), and the
+    remainder runs eagerly.  A batch whose bytes do not fit the graph rebuilds it with at least twice the capacity."""
+    loader = torch.utils.data.DataLoader(dataset, batch_size=batch_size, shuffle=False, num_workers=num_workers,
+                                         collate_fn=collater, pin_memory=True)
+    n = len(dataset)
+    dev = next(model.parameters()).device
+    graphed = None
+    i0 = 0
+    with torch.no_grad():
+        for raw in loader:
+            idx = range(i0, i0 + raw.B)
+            i0 += raw.B
+            hw = raw.S, raw.S
+            if raw.B == batch_size:
+                if graphed is not None and raw.data_bytes > graphed.max_bytes:
+                    need = max(2 * graphed.max_bytes, raw.data_bytes)
+                    # inference graphs hold no state: rebuild, after dropping every reference into the old graph's
+                    # pool (its outputs from the previous batch included), so the two pools are not held together
+                    out = cls = reg = anchors = graphed = None
+                    graphed = GraphedRawDetect(model, raw, max_bytes=need, max_candidates=MAX_CANDIDATES)
+                if graphed is None:
+                    graphed = GraphedRawDetect(model, raw, max_candidates=MAX_CANDIDATES)
+                out, scales = graphed(raw)
+                cls, reg, anchors = graphed.cls, graphed.reg, graphed.anchors
+            else:
+                images = pipeline.raw_images(raw, dev)
+                cls, reg, anchors = model._raw_predictions(images)
+                out = _ops.detect_batch(cls, reg, anchors, hw[0], hw[1], cap=_ops.candidate_cap(MAX_CANDIDATES, cls),
+                                        **model.postprocess())
+                scales = raw.scales
+            _add_batch(acc, out, cls, reg, anchors, hw, model, scales, *per_image(idx))
+            for i in idx:
+                print('{}/{}'.format(i + progress_base, n), end='\r')
+
+
+def _detect_all(dataset, model, acc, batch_size, per_image, progress_base, collater=None, num_workers=0):
     """runs the network over the whole dataset, batch_size images per pass (full batches replay one GraphedDetect, the
     remainder runs eagerly), and adds every batch to acc in image order.  per_image(indices) -> the lists acc.add()
-    takes after the scales; progress_base: the number the progress line shows for image 0."""
+    takes after the scales; progress_base: the number the progress line shows for image 0.  With a collater, the
+    dataset yields decoded samples and _detect_raw runs instead."""
+    if collater is not None:
+        return _detect_raw(dataset, model, acc, batch_size, per_image, progress_base, collater, num_workers)
     n = len(dataset)
     dev = next(model.parameters()).device
     graphed = None
@@ -169,16 +210,22 @@ def _refuse_training(model, what):
 
 
 def evaluate(generator, retinanet, iou_threshold=0.5, score_threshold=0.05, max_detections=100, save_path=None,
-             batch_size=16):
+             batch_size=16, collater=None, num_workers=0):
     """Drop-in for eval.py::evaluate (eval.py:165-257): the same generator interface (`generator[i]` -> {'img' [H,W,3],
     'scale'}, load_annotations, num_classes, label_to_name, len), the same prints and return value.  The network runs
     `batch_size` images per pass (full batches replay one GraphedDetect, the remainder runs eagerly), and selection,
-    matching and AP run on the device.  save_path is accepted and unused, as in the reference."""
+    matching and AP run on the device.  save_path is accepted and unused, as in the reference.
+
+    collater=pipeline.RawCollater(pixel_scale=255): `generator[i]` yields decoded samples ({'img': uint8 [h,w,3],
+    'annot'}, as DeviceCollater takes them) instead; a DataLoader(generator, batch_size, num_workers=num_workers,
+    collate_fn=collater, pin_memory=True) batches them and the Resizer chain runs on the device, bit-identical to the
+    host chain, inside a GraphedRawDetect.  Ground truth still comes from generator.load_annotations."""
     _refuse_training(retinanet, 'evaluate')
     n, K = len(generator), generator.num_classes()
     dev = next(retinanet.parameters()).device
     acc = VOCAccumulator(K, n, iou_threshold, score_threshold, max_detections, device=dev)
-    _detect_all(generator, retinanet, acc, batch_size, lambda idx: [[generator.load_annotations(i) for i in idx]], 1)
+    _detect_all(generator, retinanet, acc, batch_size, lambda idx: [[generator.load_annotations(i) for i in idx]], 1,
+                collater, num_workers)
     mean_ap, aps = acc.compute()
     print('\nmAP:')
     for label in range(K):
@@ -386,17 +433,18 @@ class COCOAccumulator:
         return out
 
 
-def evaluate_coco(dataset, model, threshold=0.05, batch_size=16, max_records=None):
+def evaluate_coco(dataset, model, threshold=0.05, batch_size=16, max_records=None, collater=None, num_workers=0):
     """Drop-in for eval.py::evaluate_coco (eval.py:260-338): the same dataset interface (`dataset[i]` -> {'img'
     [H,W,3], 'scale'}, image_ids, label_to_coco_label, coco, set_name, len), the same progress line, results file
     ({set_name}_bbox_results.json) and summary, with COCOeval's evaluation run on the device (no pycocotools needed).
     Returns COCOeval's 12 stats (None when there are no detections, as the reference returns early); the model is set
-    back to training mode at the end, as the reference does."""
+    back to training mode at the end, as the reference does.  collater=pipeline.RawCollater(): the dataset yields
+    decoded samples and the Resizer chain runs on the device, as in evaluate()."""
     _refuse_training(model, 'evaluate_coco')
     dev = next(model.parameters()).device
     acc = COCOAccumulator(dataset.coco, dataset.image_ids, dataset.label_to_coco_label, score_threshold=threshold,
                           max_records=max_records, device=dev)
-    _detect_all(dataset, model, acc, batch_size, lambda idx: [], 0)
+    _detect_all(dataset, model, acc, batch_size, lambda idx: [], 0, collater, num_workers)
     stats, _, _ = acc.compute()
     results = acc.results()
     if not len(results):

@@ -36,6 +36,21 @@ with more than Gcap annotations, more than Bcap images or another H x W are refu
     for idx, (images, annotations) in enumerate(train_loader):       # any batch size up to Bcap, ragged annotations
         loss = step(images, annotations, update=(idx + 1) % k == 0)
 
+Raw-batch mode, for a DataLoader whose workers decode: collate_fn=pipeline.RawCollater(...) yields RawBatch blobs
+(uint8 images, Resizer geometry, flips, annotation rows) without touching CUDA.  Built on one of them, the step is
+capacity mode with Bcap = its B, max_annotations (required) rows per image and max_bytes (default: Bcap times its
+largest image) bytes of PIXELS -- the rows have their own bound, Bcap * max_annotations.  (GraphedRawDetect has no
+max_annotations and counts rows and pixels together in its max_bytes.)  The captured region starts with the Resizer
+chain into the static images and the annotation packing (effdet_collate_pack_annots), so a call is one host-to-device
+copy of the blob and one replay.  Batches with more images, pixel bytes or rows per image are refused before anything
+is copied.
+
+    loader = DataLoader(dataset, batch_size, num_workers=4, collate_fn=RawCollater(pixel_scale=255), pin_memory=True)
+    step = None
+    for idx, raw in enumerate(loader):
+        step = step or GraphedTrainStep(model, raw, optimizer=opt, max_annotations=256)
+        loss = step(raw, update=(idx + 1) % k == 0)
+
 Training with the optimizer in the graph.  With `optimizer=FusedClipAdamW(...)` every call is one micro-step of the
 reference loop (train.py:95-133): forward, loss, backward, gradients added to the persistent accumulators that
 `p.grad` then refers to (skipped when the loss is exactly 0), and, when `update` is true and the loss is non-zero, the
@@ -81,7 +96,12 @@ class GraphedTrainStep:
     init_process_group, the DDP wrapper CONSTRUCTED inside a side-stream context, >= 11 eager warm-up iterations);
     gradients then have to flow through DDP's AccumulateGrad hooks, so the captured step calls loss.backward()."""
 
-    def __init__(self, model, images, annotations, optimizer=None, warmup=3, max_annotations=None):
+    def __init__(self, model, images, annotations=None, optimizer=None, warmup=3, max_annotations=None, max_bytes=None):
+        self.raw = None
+        if isinstance(images, pipeline.RawBatch):
+            images = self._init_raw(model, images, annotations, max_annotations, max_bytes)
+        elif annotations is None:
+            raise _ops.N.EffdetNativeError('GraphedTrainStep: example annotations are needed with example images')
         if not images.is_cuda:
             raise _ops.N.EffdetNativeError('GraphedTrainStep needs CUDA example inputs')
         self.ddp = isinstance(model, torch.nn.parallel.DistributedDataParallel)
@@ -92,7 +112,11 @@ class GraphedTrainStep:
         self.fused = isinstance(optimizer, FusedClipAdamW)
         self.static_images = images.clone()
         self.static_counts = None
-        if max_annotations is None:
+        if self.raw is not None:
+            self.static_annots = torch.full((self.raw['Bcap'], max_annotations, 5), -1.0, dtype=torch.float32,
+                                            device=images.device)
+            self.static_counts = torch.zeros((1 + self.raw['Bcap'],), dtype=torch.int32, device=images.device)
+        elif max_annotations is None:
             self.static_annots = annotations.clone()
         else:
             if isinstance(max_annotations, bool) or not isinstance(max_annotations, int) or max_annotations < 1:
@@ -123,7 +147,9 @@ class GraphedTrainStep:
             p.grad = None
         n0 = _ops.N.launch_count()
         try:
-            with torch.cuda.graph(self.graph):
+            # a raw-batch step is built while a DataLoader's pin thread allocates pinned memory: capture in
+            # thread-local mode, so that thread's CUDA calls do not invalidate this thread's capture
+            with torch.cuda.graph(self.graph, capture_error_mode='global' if self.raw is None else 'thread_local'):
                 self.static_loss = self._eager_step(params, zero=False, capture=True)
         except RuntimeError as e:
             if 'legacy stream' in str(e) or 'previous error during capture' in str(e):
@@ -140,10 +166,66 @@ class GraphedTrainStep:
             # capture recorded the weight packing without running it: eager calls derive their own until a replay
             _ops.invalidate_caches()
 
+    def _init_raw(self, model, example, annotations, max_annotations, max_bytes):
+        """raw-batch mode: the static device copy of a raw batch laid out for Bcap = example.B images, with room for
+        Bcap * max_annotations rows and max_bytes pixel bytes (pixels only, unlike GraphedRawDetect's max_bytes) ->
+        example images for the capture (zeros)"""
+        err = _ops.N.EffdetNativeError
+        if annotations is not None:
+            raise err('GraphedTrainStep(model, raw_batch, ...): a RawBatch carries its annotations; pass optimizer, '
+                      'max_annotations and max_bytes by keyword')
+        if isinstance(max_annotations, bool) or not isinstance(max_annotations, int) or max_annotations < 1:
+            raise err('GraphedTrainStep: a RawBatch example needs max_annotations, an integer >= 1, got %r'
+                      % (max_annotations,))
+        dev = next(model.parameters()).device
+        if dev.type != 'cuda':
+            raise err('GraphedTrainStep needs a model on a CUDA device')
+        Bcap = example.B
+        cap_bytes = Bcap * int(example.image_bytes.max()) if max_bytes is None else int(max_bytes)
+        _, total = pipeline.raw_layout(Bcap, Bcap * max_annotations, cap_bytes)
+        self.raw = dict(Bcap=Bcap, Gcap=max_annotations, max_bytes=cap_bytes, S=example.S,
+                        pixel_scale=example.pixel_scale, blob=torch.empty((total,), dtype=torch.uint8, device=dev))
+        self._check_raw(example)
+        self._load_raw(example)
+        return torch.zeros((Bcap, 3, example.S, example.S), device=dev)
+
+    def _check_raw(self, raw):
+        """raw-batch mode: refuse a batch that does not fit, before anything is copied or launched"""
+        err, c = _ops.N.EffdetNativeError, self.raw
+        if not isinstance(raw, pipeline.RawBatch):
+            raise err('GraphedTrainStep was built on a RawBatch: call it as step(raw_batch, update=...)')
+        if (raw.S, raw.pixel_scale) != (c['S'], c['pixel_scale']):
+            raise err('GraphedTrainStep was captured for common size %d and pixel_scale %r, got %d and %r'
+                      % (c['S'], c['pixel_scale'], raw.S, raw.pixel_scale))
+        if not 1 <= raw.B <= c['Bcap']:
+            raise err('GraphedTrainStep: a batch of %d images does not fit the capacity of %d images of the example'
+                      % (raw.B, c['Bcap']))
+        if raw.nbytes > c['max_bytes']:
+            raise err('GraphedTrainStep: a batch of %d pixel bytes does not fit max_bytes=%d; build the step with '
+                      'max_bytes=%d or more' % (raw.nbytes, c['max_bytes'], raw.nbytes))
+        if raw.max_rows > c['Gcap']:
+            raise err('GraphedTrainStep: a batch with %d annotation rows per image does not fit max_annotations=%d; '
+                      'build the step with max_annotations=%d or more' % (raw.max_rows, c['Gcap'], raw.max_rows))
+
+    def _load_raw(self, raw):
+        """raw-batch mode: the batch laid out for Bcap images (a short batch gets zero entries for the unused images,
+        in a new host blob) -> one host-to-device copy into the static blob"""
+        blob = raw.at_capacity(self.raw['Bcap'], pin=raw.blob.is_pinned()).blob
+        self.raw['blob'][:blob.numel()].copy_(blob, non_blocking=True)
+
+    def _unpack_raw(self):
+        """the head of the captured region in raw-batch mode: Normalizer -> flip -> Resizer -> pad into the static
+        images (padding images are zeros), then the annotations collated and packed with their counts"""
+        c = self.raw
+        pipeline.launch_raw_resize(self.static_images, c['blob'], c['Bcap'], c['pixel_scale'])
+        pipeline.launch_raw_pack(c['blob'], c['Bcap'], self.static_annots, self.static_counts)
+
     def _eager_step(self, params, zero=True, capture=False):
         if zero:
             for p in params:
                 p.grad = None
+        if self.raw is not None:
+            self._unpack_raw()
         inputs = [self.static_images, self.static_annots]
         if self.static_counts is not None:
             inputs.append(self.static_counts)
@@ -196,10 +278,18 @@ class GraphedTrainStep:
         annotations = annotations.to(device=self.static_annots.device, dtype=torch.float32, non_blocking=True)
         _ops.pack_annotations(annotations.contiguous(), self.static_annots, self.static_counts)
 
-    def __call__(self, images, annotations, update=True):
+    def __call__(self, images, annotations=None, update=True):
         """One micro-step.  update: run the optimizer after it (train.py:115 `(idx + 1) % k == 0`); with
-        FusedClipAdamW the update is skipped on the device when the step's loss is exactly zero."""
-        if self.static_counts is not None:
+        FusedClipAdamW the update is skipped on the device when the step's loss is exactly zero.  A step built on a
+        RawBatch is called as step(raw_batch, update=...)."""
+        if self.raw is not None:
+            if annotations is not None:
+                raise _ops.N.EffdetNativeError('GraphedTrainStep was built on a RawBatch: call it as '
+                                               'step(raw_batch, update=...)')
+            self._check_raw(images)
+        elif annotations is None:
+            raise _ops.N.EffdetNativeError('GraphedTrainStep: call it as step(images, annotations, update=...)')
+        elif self.static_counts is not None:
             self._check_batch(images, annotations)
         if self.fused:
             if self.ddp and not update:
@@ -209,7 +299,9 @@ class GraphedTrainStep:
         elif not update:
             raise _ops.N.EffdetNativeError('GraphedTrainStep: update=False (gradient accumulation) needs '
                                            'optimizer=FusedClipAdamW(...)')
-        if self.static_counts is not None:
+        if self.raw is not None:
+            self._load_raw(images)
+        elif self.static_counts is not None:
             self._load_batch(images, annotations)
         else:
             self.static_images.copy_(images, non_blocking=True)
@@ -241,6 +333,8 @@ class GraphedDetect:
     (load_state_dict, EMA copies).  The post-processing settings (threshold, iou_threshold, nms, soft_nms_sigma) are
     fixed at capture: changing one on the model makes the next call raise."""
 
+    _capture_error_mode = 'global'
+
     def __init__(self, model, images, max_candidates=8192, warmup=2):
         if model.training or model.is_training:
             raise _ops.N.EffdetNativeError('GraphedDetect needs a model in inference mode (model.eval() and '
@@ -262,7 +356,7 @@ class GraphedDetect:
         _ops.invalidate_caches()                                      # capture the weight packing and BN folding
         self.graph = torch.cuda.CUDAGraph()
         n0 = _ops.N.launch_count()
-        with torch.cuda.graph(self.graph):
+        with torch.cuda.graph(self.graph, capture_error_mode=self._capture_error_mode):
             self.cls, self.reg, self.anchors, self.out = self._run()
         self.library_launches = _ops.N.launch_count() - n0            # kernels of this library recorded into the graph
         # capture recorded the weight packing without running it: the cache entries it made hold nothing until a
@@ -388,3 +482,72 @@ class GraphedFrameDetect(GraphedDetect):
         trip = _ops.detect_batch(self.cls[b:b + 1], self.reg[b:b + 1], self.anchors, self.H, self.W, **self.post)[0]
         rows, counts = pipeline.frame_boxes(_padded(trip), self._hw[b:b + 1], self.H, self.W)
         return rows[0, :int(counts[0])].cpu().numpy()
+
+
+class GraphedRawDetect(GraphedDetect):
+    """GraphedDetect fed by raw batches (pipeline.RawCollater's output): the Resizer chain (Normalizer -> Resizer ->
+    zero pad, effdet_resize_normalize_pad) at the head of the captured region, then the network, decode and NMS (hard
+    or Soft-NMS, from model.postprocess()).
+
+        det = GraphedRawDetect(model, example_raw_batch)          # model.eval(), model.is_training False
+        out, scales = det(raw_batch)    # one host-to-device copy, one replay -> padded Detections, float64 [B] scales
+
+    The example fixes the capacity: Bcap = example.B images, and max_bytes bytes of annotation rows AND pixels together
+    (RawBatch.data_bytes, the blob after its fixed sections; default: Bcap times the example's largest image plus the
+    example's rows).  This differs from GraphedTrainStep's max_bytes, which counts pixels only because its rows are
+    bounded by max_annotations; detection reads no rows, so it bounds the blob's size alone.  A call takes 1 ..
+    Bcap images whose bytes fit; the unused capacity runs as zero padding images, whose rows of `out` are to be
+    ignored.  out is the static output of GraphedDetect: every call rewrites it."""
+
+    # built while a DataLoader's pin thread allocates pinned memory (evaluate(..., collater=)): another thread's CUDA
+    # calls must not invalidate the capture
+    _capture_error_mode = 'thread_local'
+
+    def __init__(self, model, example, max_bytes=None, max_candidates=None, warmup=2):
+        err = _ops.N.EffdetNativeError
+        if not isinstance(example, pipeline.RawBatch):
+            raise err('GraphedRawDetect needs a RawBatch example (pipeline.RawCollater output)')
+        dev = next(model.parameters()).device
+        if dev.type != 'cuda':
+            raise err('GraphedRawDetect needs a model on a CUDA device')
+        self.capacity, self.S, self.pixel_scale = example.B, example.S, example.pixel_scale
+        if max_bytes is None:
+            max_bytes = (self.capacity * int(example.image_bytes.max()) + 15) // 16 * 16 + \
+                (40 * example.rows + 15) // 16 * 16
+        self.max_bytes = int(max_bytes)
+        fixed = pipeline.raw_layout(self.capacity, 0, 0)[0]['rows']
+        self._blob = torch.empty((fixed + self.max_bytes,), dtype=torch.uint8, device=dev)
+        self._check_raw(example)
+        self._load_raw(example)
+        super().__init__(model, torch.zeros((self.capacity, 3, self.S, self.S), device=dev), max_candidates, warmup)
+
+    def _check_raw(self, raw):
+        err = _ops.N.EffdetNativeError
+        if not isinstance(raw, pipeline.RawBatch):
+            raise err('GraphedRawDetect takes RawBatch inputs (pipeline.RawCollater output)')
+        if (raw.S, raw.pixel_scale) != (self.S, self.pixel_scale):
+            raise err('GraphedRawDetect was captured for common size %d and pixel_scale %r, got %d and %r'
+                      % (self.S, self.pixel_scale, raw.S, raw.pixel_scale))
+        if not 1 <= raw.B <= self.capacity:
+            raise err('GraphedRawDetect: a batch of %d images does not fit the capacity of %d images of the example'
+                      % (raw.B, self.capacity))
+        if raw.data_bytes > self.max_bytes:
+            raise err('GraphedRawDetect: a batch of %d bytes of rows and pixels does not fit max_bytes=%d; build it '
+                      'with max_bytes=%d or more' % (raw.data_bytes, self.max_bytes, raw.data_bytes))
+
+    def _load_raw(self, raw):
+        blob = raw.at_capacity(self.capacity, pin=raw.blob.is_pinned()).blob
+        self._blob[:blob.numel()].copy_(blob, non_blocking=True)
+
+    @torch.no_grad()
+    def _run(self):
+        pipeline.launch_raw_resize(self.static_images, self._blob, self.capacity, self.pixel_scale)
+        return super()._run()
+
+    def __call__(self, raw):
+        """raw: a RawBatch of 1 .. capacity images -> (padded Detections of `capacity` rows, raw.scales)"""
+        self._check_thresholds()
+        self._check_raw(raw)
+        self._load_raw(raw)
+        self.graph.replay()
+        return self.out, raw.scales

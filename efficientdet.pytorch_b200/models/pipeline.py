@@ -44,6 +44,33 @@ def concat_pinned(imgs, staging=None):
     return flat, offs
 
 
+def check_samples(samples, S, resize, who, resize_who):
+    """the sample checks of DeviceCollater and RawCollater -> (C-contiguous uint8 images, sizes int32 [B, 2], box scales
+    float64 [B], resized sizes int32 [B, 2]).  Raises before anything is copied; who / resize_who name the caller in the
+    messages (resize_who in the refusal of 'scale', which only the Resizer path makes)."""
+    imgs = [np.ascontiguousarray(s['img']) for s in samples]
+    for im in imgs:
+        if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3 or im.shape[0] < 1 or im.shape[1] < 1 or \
+                (not resize and (im.shape[0] > S or im.shape[1] > S)):
+            raise N.EffdetNativeError('%s: images must be uint8 [h,w,3] with h,w >= 1%s, got %s %s'
+                                      % (who, '' if resize else ' and <= %d' % S, im.dtype, im.shape))
+    sizes = np.array([[im.shape[0], im.shape[1]] for im in imgs], dtype=np.int32)
+    if resize:
+        if any('scale' in s for s in samples):
+            raise N.EffdetNativeError("%s: a sample carries 'scale', but the Resizer computes each image's scale "
+                                      "itself" % resize_who)
+        geo = [resizer_geometry(int(h), int(w), S) for h, w in sizes]
+        for (h, w), (_, rh, rw) in zip(sizes, geo):
+            if rh < 1 or rw < 1:
+                raise N.EffdetNativeError('%s: a %dx%d image resizes to %dx%d at common size %d' % (who, h, w, rh, rw, S))
+        scales = np.array([g[0] for g in geo], dtype=np.float64)
+        resized = np.array([[g[1], g[2]] for g in geo], dtype=np.int32)
+    else:
+        scales = np.array([float(s.get('scale', 1.0)) for s in samples], dtype=np.float64)
+        resized = sizes
+    return imgs, sizes, scales, resized
+
+
 class DeviceCollater:
     """collate_fn replacement: call with a list of samples {'img': uint8 [h,w,3] ndarray, 'annot': [n,5] float64 ndarray,
     optional 'flip': bool, optional 'scale': float}; returns (images float32 [B,3,S,S], annotations float32 [B,G,5])
@@ -73,27 +100,8 @@ class DeviceCollater:
 
     def __call__(self, samples):
         B, S, dev = len(samples), self.S, self.device
-        imgs = [np.ascontiguousarray(s['img']) for s in samples]
-        for im in imgs:
-            if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3 or im.shape[0] < 1 or im.shape[1] < 1 or \
-                    (not self.resize and (im.shape[0] > S or im.shape[1] > S)):
-                raise N.EffdetNativeError('DeviceCollater: images must be uint8 [h,w,3] with h,w >= 1%s, got %s %s'
-                                          % ('' if self.resize else ' and <= %d' % S, im.dtype, im.shape))
-        sizes = np.array([[im.shape[0], im.shape[1]] for im in imgs], dtype=np.int32)
-        if self.resize:
-            if any('scale' in s for s in samples):
-                raise N.EffdetNativeError("DeviceCollater(resize=True): a sample carries 'scale', but the Resizer "
-                                          "computes each image's scale itself")
-            geo = [resizer_geometry(int(h), int(w), S) for h, w in sizes]
-            for (h, w), (_, rh, rw) in zip(sizes, geo):
-                if rh < 1 or rw < 1:
-                    raise N.EffdetNativeError('DeviceCollater: a %dx%d image resizes to %dx%d at common size %d'
-                                              % (h, w, rh, rw, S))
-            scales = np.array([g[0] for g in geo], dtype=np.float64)
-            resized = np.array([[g[1], g[2]] for g in geo], dtype=np.int32)
-        else:
-            scales = np.array([float(s.get('scale', 1.0)) for s in samples], dtype=np.float64)
-            resized = sizes
+        imgs, sizes, scales, resized = check_samples(samples, S, self.resize, 'DeviceCollater',
+                                                     'DeviceCollater(resize=True)')
         flat, offs = concat_pinned(imgs)
         flips = np.array([1 if s.get('flip') else 0 for s in samples], dtype=np.uint8)
         anns = [np.asarray(s['annot'], dtype=np.float64).reshape(-1, 5) for s in samples]
@@ -119,6 +127,175 @@ class DeviceCollater:
         if self.return_scales:
             return out, ann, scales
         return out, ann
+
+
+# ---- raw batches: what DataLoader workers hand to the graphed steps ---------------------------------------------------
+RAW_HEADER = 8          # int64 header entries: B, pixel bytes, rows, layout capacity, common size, pixel scale, 0, 0
+_MEAN64 = (ctypes.c_double * 3)(*MEAN)
+_STD64 = (ctypes.c_double * 3)(*STD)
+
+
+def raw_layout(capacity, rows, nbytes):
+    """byte offset of every section of a raw batch whose per-image sections hold `capacity` images, with `rows`
+    annotation rows and `nbytes` pixel bytes -> (dict name -> offset, total bytes).  Every section starts on a 16-byte
+    boundary; the sections up to 'rows' depend on the capacity alone."""
+    sizes = [('header', 8 * RAW_HEADER), ('offsets', 8 * capacity), ('hw', 8 * capacity), ('resized_hw', 8 * capacity),
+             ('flips', capacity), ('scales', 8 * capacity), ('row_offsets', 4 * (capacity + 1)), ('rows', 40 * rows),
+             ('pixels', nbytes)]
+    off, at = {}, 0
+    for name, n in sizes:
+        off[name] = at
+        at += (n + 15) // 16 * 16
+    return off, at
+
+
+_SECTIONS = {'header': (torch.int64, RAW_HEADER), 'offsets': (torch.int64, 1), 'hw': (torch.int32, 2),
+             'resized_hw': (torch.int32, 2), 'flips': (torch.uint8, 1), 'scales': (torch.float64, 1),
+             'row_offsets': (torch.int32, 1)}
+
+
+def raw_section(blob, capacity, name):
+    """a typed view of one fixed section of a raw batch (host or device) laid out for `capacity` images: header int64
+    [8], offsets int64 [cap], hw / resized_hw int32 [cap, 2], flips uint8 [cap], scales float64 [cap], row_offsets
+    int32 [cap + 1]"""
+    off, _ = raw_layout(capacity, 0, 0)
+    dtype, width = _SECTIONS[name]
+    n = RAW_HEADER if name == 'header' else (capacity + 1 if name == 'row_offsets' else capacity * width)
+    v = blob[off[name]:off[name] + n * dtype.itemsize].view(dtype)
+    return v.reshape(capacity, width) if width == 2 else v
+
+
+def _assemble(capacity, S, pixel_scale, sizes, resized, flips, scales, counts, rows, pixels, pin=False):
+    """one raw batch blob laid out for `capacity` >= B images: entries b >= B of the per-image sections are zero (an
+    image with h = 0 is padding to the resize kernel).  pixels: a list of uint8 arrays, back to back."""
+    B = len(sizes)
+    image_bytes = sizes[:, 0].astype(np.int64) * sizes[:, 1] * 3
+    nbytes, R = int(image_bytes.sum()), int(counts.sum())
+    off, total = raw_layout(capacity, R, nbytes)
+    blob = torch.empty((total,), dtype=torch.uint8, pin_memory=pin)
+    a = blob.numpy()
+    p0 = off['pixels']
+    a[:p0] = 0                                                   # header tail, row slots and padding: deterministic
+    a[p0 + nbytes:] = 0
+
+    def put(name, arr):
+        arr = np.ascontiguousarray(arr).reshape(-1).view(np.uint8)
+        a[off[name]:off[name] + arr.size] = arr
+
+    put('header', np.array([B, nbytes, R, capacity, S, pixel_scale or 1, 0, 0], np.int64))
+    put('offsets', p0 + np.concatenate([[0], np.cumsum(image_bytes)[:-1]]).astype(np.int64))   # from the blob's start
+    put('hw', sizes.astype(np.int32))
+    put('resized_hw', resized.astype(np.int32))
+    put('flips', flips.astype(np.uint8))
+    put('scales', scales.astype(np.float64))
+    put('row_offsets', np.concatenate([[0], np.cumsum(counts)]).astype(np.int32))
+    put('rows', rows.astype(np.float64))
+    np.concatenate([np.asarray(p).reshape(-1) for p in pixels] or [np.zeros(0, np.uint8)], out=a[p0:p0 + nbytes])
+    return RawBatch(blob, capacity, S, pixel_scale, counts, image_bytes, scales)
+
+
+class RawBatch:
+    """A batch as DataLoader workers can build it without CUDA: decoded uint8 images, the Resizer's geometry, the flips
+    and the ragged annotation rows in ONE contiguous uint8 host tensor (`blob`), so that a graphed step needs one
+    host-to-device copy.  Sections, each 16-byte aligned (raw_layout): header int64 [8] (B, pixel bytes, rows, layout
+    capacity, common size, pixel scale), byte offsets int64 [cap] (from the blob's start), hw and resized_hw int32
+    [cap, 2], flips uint8 [cap], Resizer scales float64 [cap], row offsets int32 [cap + 1], rows float64 [R, 5], pixels.
+    A collated batch is laid out for its own B images (capacity == B).
+
+    Host-side facts, for the capacity checks without a device read: B, counts (rows per image), image_bytes, nbytes,
+    and scales (float64 [B], eval.py's data['scale'], as VOCAccumulator.add() takes them)."""
+
+    def __init__(self, blob, capacity, S, pixel_scale, counts, image_bytes, scales):
+        self.blob = blob
+        self.capacity, self.S, self.pixel_scale = int(capacity), int(S), pixel_scale
+        self.counts = np.asarray(counts, dtype=np.int32)
+        self.image_bytes = np.asarray(image_bytes, dtype=np.int64)
+        self.scales = np.asarray(scales, dtype=np.float64)
+        self.B, self.nbytes, self.rows = len(self.counts), int(self.image_bytes.sum()), int(self.counts.sum())
+
+    def __len__(self):
+        return self.B
+
+    @property
+    def max_rows(self):
+        """the most annotation rows of one image (what max_annotations must hold)"""
+        return int(self.counts.max()) if self.B else 0
+
+    @property
+    def data_bytes(self):
+        """bytes of the rows and pixel sections: the blob's size after its fixed, capacity-sized sections"""
+        return (40 * self.rows + 15) // 16 * 16 + (self.nbytes + 15) // 16 * 16
+
+    def section(self, name):
+        return raw_section(self.blob, self.capacity, name)
+
+    def pin_memory(self):
+        """a copy in pinned memory (DataLoader(pin_memory=True) calls this in its pin thread)"""
+        return RawBatch(self.blob.pin_memory(), self.capacity, self.S, self.pixel_scale, self.counts, self.image_bytes,
+                        self.scales)
+
+    def at_capacity(self, capacity, pin=False):
+        """the same batch laid out for `capacity` >= B images (zero entries for the unused ones): what a graph captured
+        for `capacity` images reads"""
+        if capacity == self.capacity:
+            return self
+        B = self.B
+        off, _ = raw_layout(self.capacity, self.rows, self.nbytes)
+        a = self.blob.numpy()
+        rows = a[off['rows']:off['rows'] + 40 * self.rows].view(np.float64).reshape(-1, 5)
+        return _assemble(capacity, self.S, self.pixel_scale, self.section('hw')[:B].numpy(),
+                         self.section('resized_hw')[:B].numpy(), self.section('flips')[:B].numpy(), self.scales,
+                         self.counts, rows, [a[off['pixels']:off['pixels'] + self.nbytes]], pin=pin)
+
+
+class RawCollater:
+    """collate_fn for DataLoader workers: takes DeviceCollater(resize=True)'s samples ({'img': uint8 [h,w,3], 'annot':
+    float64 [n,5], optional 'flip'}, no 'scale'), refuses what it refuses, and returns a RawBatch.  It never touches
+    CUDA, so it runs in forked workers after the parent has initialised CUDA; GraphedTrainStep / GraphedRawDetect run
+    the Normalizer -> Augmenter flip -> Resizer -> collater chain on the device, bit-identical to DeviceCollater.
+    pixel_scale: None (COCO, float32(u8)) or 255 (VOC, float32(u8) / 255), as DeviceCollater."""
+
+    def __init__(self, common_size=512, pixel_scale=None):
+        if pixel_scale not in (None, 255):
+            raise N.EffdetNativeError('RawCollater: pixel_scale must be None (COCO) or 255 (VOC), got %r' % (pixel_scale,))
+        self.S, self.pixel_scale = int(common_size), pixel_scale
+
+    def __call__(self, samples):
+        imgs, sizes, scales, resized = check_samples(samples, self.S, True, 'RawCollater', 'RawCollater')
+        flips = np.array([1 if s.get('flip') else 0 for s in samples], dtype=np.uint8)
+        anns = [np.asarray(s['annot'], dtype=np.float64).reshape(-1, 5) for s in samples]
+        counts = np.array([a.shape[0] for a in anns], dtype=np.int32)
+        rows = np.concatenate(anns, axis=0) if counts.sum() else np.zeros((0, 5))
+        return _assemble(len(samples), self.S, self.pixel_scale, sizes, resized, flips, scales, counts, rows, imgs)
+
+
+def launch_raw_resize(out, blob, capacity, pixel_scale):
+    """effdet_resize_normalize_pad of a raw batch in device memory laid out for `capacity` images into out float32
+    [capacity, 3, S, S]; the geometry arguments point into the blob, and padding entries (h = 0) write zeros"""
+    S = out.shape[2]
+    sec = lambda name: raw_section(blob, capacity, name)               # noqa: E731
+    N.call('effdet_resize_normalize_pad', out, N.ptr(blob), N.ptr(sec('offsets')), N.ptr(sec('hw')),
+           N.ptr(sec('resized_hw')), N.ptr(sec('flips')), N.f32(out), capacity, S, pixel_scale or 1, _MEAN64, _STD64,
+           nbytes=float(blob.numel() + 4 * out.numel()))
+
+
+def launch_raw_pack(blob, capacity, annots, counts):
+    """effdet_collate_pack_annots of a raw batch in device memory laid out for `capacity` images into the static table
+    annots float32 [capacity, Gcap, 5] and counts int32 [1 + capacity]"""
+    sec = lambda name: raw_section(blob, capacity, name)               # noqa: E731
+    rows = blob[raw_layout(capacity, 0, 0)[0]['rows']:]
+    N.call('effdet_collate_pack_annots', annots, N.ptr(sec('header')), N.ptr(rows), N.ptr(sec('row_offsets')),
+           N.ptr(sec('scales')), N.ptr(sec('flips')), N.ptr(sec('hw')), N.f32(annots), N.ptr(counts), capacity,
+           annots.shape[1])
+
+
+def raw_images(raw, device='cuda:0'):
+    """the images of a raw batch on the device, eagerly: float32 [B, 3, S, S], bit-identical to DeviceCollater(S,
+    resize=True, pixel_scale=raw.pixel_scale)"""
+    blob = raw.blob.to(device, non_blocking=raw.blob.is_pinned())
+    out = torch.empty((raw.capacity, 3, raw.S, raw.S), device=blob.device, dtype=torch.float32)
+    launch_raw_resize(out, blob, raw.capacity, raw.pixel_scale)
+    return out[:raw.B]
 
 
 def select_detections(scores, labels, boxes, scale, score_threshold=0.05, max_detections=100, num_classes=80):

@@ -466,6 +466,15 @@ int effdet_normalize_pad(const uint8_t* pixels, const int64_t* offsets, const in
                          effdet_stream_t stream);
 int effdet_collate_annots(const double* rows, const int32_t* row_off, const double* scale, const uint8_t* flip,
                           const int32_t* width, float* out, int B, int G, int device, effdet_stream_t stream);
+/* effdet_collate_annots followed by effdet_pack_annots, bit for bit, in one launch and with no host read, for a raw batch
+ * (models/pipeline.py RawBatch) in device memory: B = header[0] (1..Bcap) images, image b owns rows row_off[b] ..
+ * row_off[b+1] (at most Gcap of them), flip [Bcap], hw [Bcap,2] (the width is the flip's `cols`), scale [Bcap] float64.
+ * out [Bcap,Gcap,5] float32: per image its rows whose float32 label is not -1, flipped and scaled, in order, then -1
+ * rows; counts [1+Bcap]: counts[0] = B, counts[1+b] = rows kept, 0 for b >= B.  Refused before the launch: a null
+ * pointer, Bcap outside 1..65535, Gcap < 1.  Whether a batch fits is the caller's check (RawBatch holds the counts). */
+int effdet_collate_pack_annots(const int64_t* header, const double* rows, const int32_t* row_off, const double* scale,
+                               const uint8_t* flip, const int32_t* hw, float* out, int32_t* counts, int Bcap, int Gcap,
+                               int device, effdet_stream_t stream);
 /* The same input step with Resizer's cv2.resize (datasets/augmentation.py:94-115,118-150): images of any size h, w >= 1,
  * image b resized (after the flip) to resized_hw[2b] x resized_hw[2b+1] (1 .. S each) by OpenCV's generic INTER_LINEAR
  * for CV_64FC3 on the float64 normalized image, zero padded to S x S, cast to float32 once.  pixel_scale selects the
