@@ -26,6 +26,11 @@
 //   * residency, from n: slices of ceil(n/cs) <= kSlice candidates live in shared memory; larger ones (only possible
 //     when cap > kMaxCluster*kSlice, where the workspace is non-empty) live in the global workspace [B][cap] of
 //     (float4 box, float score, int32 anchor), which stays in L2 for realistic sizes.
+//
+// Per-class Soft-NMS (kClasses): picks still go in the global (score, anchor) order, but a pick decays only the live
+// candidates of its own class (classes [B,A]); the others stay live and unchanged.  Restricted to one class, the picks
+// are Soft-NMS run on that class alone.  A shared-memory slot then also holds the candidate's class (28 bytes a slot);
+// a slice in the global workspace reads it from classes, so the workspace is the agnostic kernel's.
 #include <cooperative_groups.h>
 
 #include "common.cuh"
@@ -83,6 +88,7 @@ __device__ __forceinline__ uint64_t shfl_min_u64(uint64_t v) {
     return v;
 }
 
+template <bool kClasses>
 __global__ void __launch_bounds__(kSoftThreads, 1) soft_nms_kernel(
     const float* __restrict__ boxes, const float* __restrict__ scores, const int32_t* __restrict__ classes,
     const uint64_t* __restrict__ keys, const int32_t* __restrict__ count, int A, int npad, int cap, int method,
@@ -93,6 +99,7 @@ __global__ void __launch_bounds__(kSoftThreads, 1) soft_nms_kernel(
     float4* s_box = reinterpret_cast<float4*>(soft_smem);
     float* s_score = reinterpret_cast<float*>(s_box + kSlice);
     int32_t* s_anchor = reinterpret_cast<int32_t*>(s_score + kSlice);
+    int32_t* s_class = s_anchor + kSlice;          // kClasses only
     __shared__ SoftSlot slot[2];
     __shared__ uint64_t w_key[kSoftWarps];
     __shared__ float4 w_box[kSoftWarps];
@@ -126,11 +133,14 @@ __global__ void __launch_bounds__(kSoftThreads, 1) soft_nms_kernel(
     float4* box = s_box;
     float* score = s_score;
     int32_t* anchor = s_anchor;
+    int32_t* klass = s_class;                      // kClasses: the slice's classes, null when read from `classes`
     if (per > kSlice) {                            // global residency: the host guarantees the workspace
         box = ws_box + b * cap + lo;
         score = ws_score + b * cap + lo;
         anchor = ws_anchor + b * cap + lo;
+        klass = nullptr;
     }
+    const int32_t* cb = classes + b * A;
     const float* bx = boxes + b * A * 4;
     const float* sc = scores + b * A;
     const uint64_t* kb = keys + b * npad;
@@ -146,6 +156,9 @@ __global__ void __launch_bounds__(kSoftThreads, 1) soft_nms_kernel(
         box[i] = v;
         score[i] = s;
         anchor[i] = a;
+        if constexpr (kClasses) {
+            if (klass) klass[i] = cb[a];
+        }
         const bool ok = s > threshold;             // false only through the C ABI, with a higher threshold
         const uint64_t k = ok ? soft_key(s, a) : ~0ull;
         if (k < best) { best = k; bbox = v; }
@@ -198,9 +211,12 @@ __global__ void __launch_bounds__(kSoftThreads, 1) soft_nms_kernel(
                 const int i = base + tid;
                 float4 v;
                 float s = 0.f;
-                int a = 0;
+                int a = 0, c = 0;
                 const bool keep = i < len && score[i] > threshold;
                 if (keep) { v = box[i]; s = score[i]; a = anchor[i]; }
+                if constexpr (kClasses) {
+                    if (keep && klass) c = klass[i];
+                }
                 const uint32_t bal = __ballot_sync(0xffffffffu, keep);
                 if (lane == 0) w_cnt[warp] = __popc(bal);
                 __syncthreads();
@@ -215,6 +231,9 @@ __global__ void __launch_bounds__(kSoftThreads, 1) soft_nms_kernel(
                     box[j] = v;
                     score[j] = s;
                     anchor[j] = a;
+                    if constexpr (kClasses) {
+                        if (klass) klass[j] = c;
+                    }
                 }
                 out += sum;
                 __syncthreads();
@@ -224,6 +243,8 @@ __global__ void __launch_bounds__(kSoftThreads, 1) soft_nms_kernel(
         // 4. decay the slice against the winner; the winner itself leaves it
         best = ~0ull;
         live = 0;
+        int32_t wc = 0;
+        if constexpr (kClasses) wc = cb[wa];
         for (int i = tid; i < len; i += kSoftThreads) {
             float s = score[i];
             if (!(s > threshold)) continue;
@@ -233,7 +254,9 @@ __global__ void __launch_bounds__(kSoftThreads, 1) soft_nms_kernel(
                 score[i] = __int_as_float(0x7fc00000);      // NaN: never > threshold
                 continue;
             }
-            const float ov = soft_iou(wbox, v);
+            bool same = true;
+            if constexpr (kClasses) same = (klass ? klass[i] : cb[a]) == wc;
+            const float ov = same ? soft_iou(wbox, v) : 0.f;
             if (ov != 0.f) {
                 s = __fmul_rn(s, soft_weight(ov, method, iou_threshold, sigma));
                 score[i] = s;
@@ -259,7 +282,9 @@ static int soft_cluster_size(int cap) {
     return cs;
 }
 
-static size_t soft_smem_bytes() { return (size_t)kSlice * (sizeof(float4) + sizeof(float) + sizeof(int32_t)); }
+static size_t soft_smem_bytes(bool with_classes) {
+    return (size_t)kSlice * (sizeof(float4) + sizeof(float) + sizeof(int32_t) + (with_classes ? sizeof(int32_t) : 0));
+}
 
 // the global slices: [B][cap] boxes, then scores, then anchors, rounded up to 16 bytes; empty unless some image can
 // need them
@@ -272,10 +297,11 @@ static long long soft_workspace_bytes(int B, int cap) {
 static int soft_nms_launch(const float* boxes, const float* scores, const int32_t* classes, const uint64_t* keys,
                            const int32_t* count, int B, int A, int npad, int cap, int method, double iou_threshold,
                            double sigma, float threshold, void* ws, float* out_scores, int64_t* out_classes,
-                           float* out_boxes, int32_t* out_count, cudaStream_t st) {
+                           float* out_boxes, int32_t* out_count, cudaStream_t st, bool with_classes = false) {
     const int cs = soft_cluster_size(cap);
-    const size_t smem = soft_smem_bytes();
-    cudaError_t e = cudaFuncSetAttribute(soft_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const size_t smem = soft_smem_bytes(with_classes);
+    auto kernel = with_classes ? soft_nms_kernel<true> : soft_nms_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return fail(EFFDET_ERR_LAUNCH, "soft_nms: smem opt-in: %s", cudaGetErrorString(e));
     float4* ws_box = nullptr;
     float* ws_score = nullptr;
@@ -297,7 +323,7 @@ static int soft_nms_launch(const float* boxes, const float* scores, const int32_
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    e = cudaLaunchKernelEx(&cfg, soft_nms_kernel, boxes, scores, classes, keys, count, A, npad, cap, method,
+    e = cudaLaunchKernelEx(&cfg, kernel, boxes, scores, classes, keys, count, A, npad, cap, method,
                            iou_threshold, sigma, threshold, ws_box, ws_score, ws_anchor, out_scores,
                            (long long*)out_classes, out_boxes, out_count);
     if (e != cudaSuccess) {
@@ -320,30 +346,44 @@ extern "C" int64_t effdet_soft_nms_workspace(int B, int cap) {
     return soft_workspace_bytes(B, cap);
 }
 
+// the refusals of effdet_soft_nms_batch and effdet_soft_nms_batch_classes, named after the entry `fn`
+#define SOFT_NMS_CHECKS(fn)                                                                                            \
+    EFFDET_REQUIRE(boxes && scores && classes && keys && count && out_scores && out_classes && out_boxes && out_count,  \
+                   fn ": null tensor");                                                                                \
+    SOFT_NMS_LIMITS(fn, B, cap);                                                                                       \
+    EFFDET_REQUIRE(A > 0 && npad >= A && (npad & (npad - 1)) == 0,                                                     \
+                   fn ": npad=%d must be a power of two >= A=%d", npad, A);                                            \
+    EFFDET_REQUIRE(cap <= A, fn ": cap=%d must be in [1, A=%d]", cap, A);                                              \
+    EFFDET_REQUIRE(method == EFFDET_SOFT_NMS_LINEAR || method == EFFDET_SOFT_NMS_GAUSSIAN,                             \
+                   fn ": method=%d must be EFFDET_SOFT_NMS_LINEAR (1) or EFFDET_SOFT_NMS_GAUSSIAN (2)", method);       \
+    EFFDET_REQUIRE(method != EFFDET_SOFT_NMS_LINEAR || (iou_threshold >= 0.0 && iou_threshold <= 1.0),                 \
+                   fn ": iou_threshold=%g must be in [0, 1] for the linear method", iou_threshold);                    \
+    EFFDET_REQUIRE(sigma > 0.0 && sigma <= 1.7976931348623157e308, fn ": sigma=%g must be finite and > 0", sigma);     \
+    const long long need = soft_workspace_bytes(B, cap);                                                               \
+    EFFDET_REQUIRE(workspace_bytes >= need, fn ": workspace of %lld bytes, %lld needed", (long long)workspace_bytes,    \
+                   need);                                                                                              \
+    EFFDET_REQUIRE(need == 0 || workspace, fn ": null workspace, %lld bytes needed", need);                            \
+    EFFDET_REQUIRE(aligned16(boxes) && aligned16(out_boxes) && aligned16(workspace),                                   \
+                   fn ": boxes, out_boxes and workspace must be 16-byte aligned");                                     \
+    EFFDET_DEVICE(device)
+
 extern "C" int effdet_soft_nms_batch(const float* boxes, const float* scores, const int32_t* classes,
                                      const uint64_t* keys, const int32_t* count, int B, int A, int npad, int cap,
                                      int method, double iou_threshold, double sigma, float threshold, void* workspace,
                                      int64_t workspace_bytes, float* out_scores, int64_t* out_classes, float* out_boxes,
                                      int32_t* out_count, int device, effdet_stream_t stream) {
-    EFFDET_REQUIRE(boxes && scores && classes && keys && count && out_scores && out_classes && out_boxes && out_count,
-                   "soft_nms_batch: null tensor");
-    SOFT_NMS_LIMITS("soft_nms_batch", B, cap);
-    EFFDET_REQUIRE(A > 0 && npad >= A && (npad & (npad - 1)) == 0,
-                   "soft_nms_batch: npad=%d must be a power of two >= A=%d", npad, A);
-    EFFDET_REQUIRE(cap <= A, "soft_nms_batch: cap=%d must be in [1, A=%d]", cap, A);
-    EFFDET_REQUIRE(method == EFFDET_SOFT_NMS_LINEAR || method == EFFDET_SOFT_NMS_GAUSSIAN,
-                   "soft_nms_batch: method=%d must be EFFDET_SOFT_NMS_LINEAR (1) or EFFDET_SOFT_NMS_GAUSSIAN (2)", method);
-    EFFDET_REQUIRE(method != EFFDET_SOFT_NMS_LINEAR || (iou_threshold >= 0.0 && iou_threshold <= 1.0),
-                   "soft_nms_batch: iou_threshold=%g must be in [0, 1] for the linear method", iou_threshold);
-    EFFDET_REQUIRE(sigma > 0.0 && sigma <= 1.7976931348623157e308, "soft_nms_batch: sigma=%g must be finite and > 0",
-                   sigma);
-    const long long need = soft_workspace_bytes(B, cap);
-    EFFDET_REQUIRE(workspace_bytes >= need, "soft_nms_batch: workspace of %lld bytes, %lld needed",
-                   (long long)workspace_bytes, need);
-    EFFDET_REQUIRE(need == 0 || workspace, "soft_nms_batch: null workspace, %lld bytes needed", need);
-    EFFDET_REQUIRE(aligned16(boxes) && aligned16(out_boxes) && aligned16(workspace),
-                   "soft_nms_batch: boxes, out_boxes and workspace must be 16-byte aligned");
-    EFFDET_DEVICE(device);
+    SOFT_NMS_CHECKS("soft_nms_batch");
     return soft_nms_launch(boxes, scores, classes, keys, count, B, A, npad, cap, method, iou_threshold, sigma, threshold,
                            workspace, out_scores, out_classes, out_boxes, out_count, (cudaStream_t)stream);
+}
+
+extern "C" int effdet_soft_nms_batch_classes(const float* boxes, const float* scores, const int32_t* classes,
+                                             const uint64_t* keys, const int32_t* count, int B, int A, int npad,
+                                             int cap, int method, double iou_threshold, double sigma, float threshold,
+                                             void* workspace, int64_t workspace_bytes, float* out_scores,
+                                             int64_t* out_classes, float* out_boxes, int32_t* out_count, int device,
+                                             effdet_stream_t stream) {
+    SOFT_NMS_CHECKS("soft_nms_batch_classes");
+    return soft_nms_launch(boxes, scores, classes, keys, count, B, A, npad, cap, method, iou_threshold, sigma, threshold,
+                           workspace, out_scores, out_classes, out_boxes, out_count, (cudaStream_t)stream, true);
 }

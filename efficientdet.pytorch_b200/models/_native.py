@@ -163,6 +163,9 @@ SIGNATURES = {
     'effdet_nms_batch_chunked': [_P, _P, _P] + [_INT] * 5 + [ctypes.c_double, _P, _I64, _P, _P] + _TAIL,
     'effdet_gather_detections_batch': [_P, _P, _P, _P, _P, _INT, _INT, _INT, _P, _P, _P] + _TAIL,
     'effdet_soft_nms_batch': [_P] * 5 + [_INT] * 5 + [ctypes.c_double] * 2 + [_F, _P, _I64] + [_P] * 4 + _TAIL,
+    'effdet_soft_nms_batch_classes': [_P] * 5 + [_INT] * 5 + [ctypes.c_double] * 2 + [_F, _P, _I64] + [_P] * 4 + _TAIL,
+    'effdet_nms_batch_chunked_classes': [_P] * 4 + [_INT] * 5 + [ctypes.c_double, _P, _I64, _P, _P] + _TAIL,
+    'effdet_detect_topk_batch': [_P] * 3 + [_INT] * 3 + [_F] * 3 + [_INT, _INT, _P, _I64] + [_P] * 5 + _TAIL,
     'effdet_multi_sumsq': [_P, _P, _P, _P, _INT, _INT, _P] + _TAIL,
     'effdet_multi_clip_adamw': [_P] * 7 + [_INT, _INT, _P] + [_F] * 8 + [_INT] + _TAIL,
     'effdet_multi_accumulate': [_P] * 5 + [_INT, _INT] + [_P] * 3 + _TAIL,
@@ -189,7 +192,8 @@ PLAIN = {'effdet_version': (ctypes.c_int, []), 'effdet_conv_tc_kpad': (ctypes.c_
          'effdet_voc_ap_workspace': (ctypes.c_int64, [ctypes.c_int] * 2),
          'effdet_coco_accumulate_workspace': (ctypes.c_int64, [ctypes.c_int] * 3),
          'effdet_nms_chunked_workspace': (ctypes.c_int64, [ctypes.c_int] * 3),
-         'effdet_soft_nms_workspace': (ctypes.c_int64, [ctypes.c_int] * 2)}
+         'effdet_soft_nms_workspace': (ctypes.c_int64, [ctypes.c_int] * 2),
+         'effdet_detect_topk_workspace': (ctypes.c_int64, [ctypes.c_int] * 4)}
 
 _lib = None
 _lock = threading.Lock()

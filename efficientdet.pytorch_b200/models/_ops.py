@@ -9,6 +9,7 @@ NCHW tensor with channels_last strides (zero-copy ``permute`` views).
 """
 import collections
 import math
+import numbers
 import os
 import weakref
 
@@ -1090,9 +1091,12 @@ NMS_CHUNK = 4096
 Detections = collections.namedtuple('Detections', 'scores classes boxes count')
 
 
-def candidate_cap(max_candidates, cls):
-    """the fixed cap detect_batch gets for cls [B,A,K]: max_candidates clamped to A, or A for None"""
+def candidate_cap(max_candidates, cls, class_nms='agnostic', pre_nms_top_k=5000):
+    """the fixed cap detect_batch gets for cls [B,A,K]: max_candidates clamped to A, or A for None; in 'multi_label'
+    mode clamped to the k' = min(pre_nms_top_k, A*K) candidate slots instead (detect_batch applies the same clamp)"""
     A = cls.shape[1]
+    if class_nms == 'multi_label':
+        A = multi_label_slots(A, cls.shape[2], pre_nms_top_k)
     return A if max_candidates is None else min(int(max_candidates), A)
 
 
@@ -1123,6 +1127,31 @@ def nms_method(nms, sigma, iou_threshold):
     return NMS_METHODS[nms]
 
 
+CLASS_NMS = ('agnostic', 'per_class', 'multi_label')
+
+
+def check_class_nms(class_nms, pre_nms_top_k):
+    """refuses a class_nms that is not one of CLASS_NMS and a pre_nms_top_k that is not an int >= 1 (checked in every
+    mode, used in 'multi_label' only)"""
+    if not isinstance(class_nms, str) or class_nms not in CLASS_NMS:
+        raise N.EffdetNativeError("class_nms=%r must be one of 'agnostic', 'per_class', 'multi_label'" % (class_nms,))
+    if isinstance(pre_nms_top_k, bool) or not isinstance(pre_nms_top_k, numbers.Integral) or pre_nms_top_k < 1:
+        raise N.EffdetNativeError('pre_nms_top_k=%r must be an int >= 1' % (pre_nms_top_k,))
+
+
+def multi_label_slots(A, K, pre_nms_top_k):
+    """candidate slots per image in 'multi_label' mode: k' = min(pre_nms_top_k, A*K)"""
+    return min(int(pre_nms_top_k), A * K)
+
+
+def _topk_workspace(B, A, K, top_k):
+    """bytes of effdet_detect_topk_batch's workspace"""
+    n = int(N.load().effdet_detect_topk_workspace(B, A, K, top_k))
+    if n < 0:
+        raise N.EffdetNativeError('detect_batch: %s' % N.last_error())
+    return n
+
+
 def _soft_nms_workspace(B, cap):
     """bytes of effdet_soft_nms_batch's workspace, a multiple of 16 (0 up to cap = 32768)"""
     n = int(N.load().effdet_soft_nms_workspace(B, cap))
@@ -1131,13 +1160,20 @@ def _soft_nms_workspace(B, cap):
     return n
 
 
-def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=None, nms='hard', sigma=0.5):
+def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=None, nms='hard', sigma=0.5,
+                 class_nms='agnostic', pre_nms_top_k=5000):
     """Decode + clip + class max + threshold + greedy NMS of every image of cls [B,A,K] / reg [B,A,4], one set of
     launches for the whole batch (the reference does this for image 0 only, models/efficientdet.py:73-86).
 
     nms='hard' is torchvision's greedy NMS at iou_threshold.  nms='linear' / 'gaussian' is Soft-NMS
     (effdet_soft_nms_batch): 'linear' decays by 1 - IoU above iou_threshold, 'gaussian' by exp(-IoU^2 / sigma); the
     returned scores are the decayed ones, in pick order (non-increasing), all above threshold.
+
+    class_nms='agnostic' is the reference's NMS: one label per anchor (its class max) and suppression across classes.
+    'per_class' keeps those candidates but a box suppresses (or, with Soft-NMS, decays) only boxes of its own class: the
+    hard keep sets are torchvision's _batched_nms_vanilla, rows in (score desc, anchor asc) order.  'multi_label' makes
+    every (anchor a, class k) pair with cls[b, a, k] > threshold a candidate, keeps the best
+    k' = min(pre_nms_top_k, A*K) of them (ties: lower a*K + k) and runs per-class NMS on those; cap is clamped to k'.
 
     cap=None: reads the B candidate counts once to set cap = their maximum and the B kept counts once to slice the
     results -> list of B triples [scores[K_b], classes[K_b] int64, boxes[K_b,4]] on the device (empty tensors when no
@@ -1146,11 +1182,16 @@ def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=
     classes [B,C] int64, boxes [B,C,4], count [B] int32), rows past count[b] zero; count[b] == -1 when image b has
     more than C candidates (its rows are then all zero)."""
     method = nms_method(nms, sigma, iou_threshold)
+    check_class_nms(class_nms, pre_nms_top_k)
     check_cuda_f32(cls, 'classifications')
     check_cuda_f32(reg, 'regressions')
     cls, reg = _contig(cls), _contig(reg)
     B, A, K = cls.shape
     anchors = _contig(anchors.view(-1, 4))
+    if class_nms == 'multi_label':
+        A = multi_label_slots(A, K, pre_nms_top_k)           # from here on the candidate slots stand for the anchors
+        if cap is not None:
+            cap = min(cap, A)
     npad = 1 << (A - 1).bit_length()
     dev = cls.device
     boxes = _empty((B, A, 4), cls)
@@ -1158,9 +1199,17 @@ def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=
     classes = torch.empty((B, A), device=dev, dtype=torch.int32)
     keys = torch.empty((B, npad), device=dev, dtype=torch.int64)
     count = torch.empty((B,), device=dev, dtype=torch.int32)
-    N.call('effdet_detect_candidates_batch', cls, N.f32(cls), N.f32(reg), N.f32(anchors), N.f32(boxes), N.f32(scores),
-           classes.data_ptr(), keys.data_ptr(), count.data_ptr(), B, A, K, npad, float(img_w), float(img_h),
-           float(threshold))
+    if class_nms == 'multi_label':
+        ws_bytes = _topk_workspace(B, cls.shape[1], K, A)
+        ws = torch.empty((ws_bytes // 8,), device=dev, dtype=torch.int64)
+        N.call('effdet_detect_topk_batch', cls, N.f32(cls), N.f32(reg), N.f32(anchors), B, cls.shape[1], K,
+               float(img_w), float(img_h), float(threshold), A, npad, ws.data_ptr(), ws_bytes, N.f32(boxes),
+               N.f32(scores), classes.data_ptr(), keys.data_ptr(), count.data_ptr())
+    else:
+        N.call('effdet_detect_candidates_batch', cls, N.f32(cls), N.f32(reg), N.f32(anchors), N.f32(boxes),
+               N.f32(scores), classes.data_ptr(), keys.data_ptr(), count.data_ptr(), B, A, K, npad, float(img_w),
+               float(img_h), float(threshold))
+    per_class = class_nms != 'agnostic'
     eager = cap is None
     if eager:
         cap = int(count.max().item())                # host read 1 of 2: sizes the NMS workspace and the outputs
@@ -1174,20 +1223,22 @@ def detect_batch(cls, reg, anchors, img_h, img_w, threshold, iou_threshold, cap=
     if method:
         ws_bytes = _soft_nms_workspace(B, cap)
         ws = torch.empty((max(ws_bytes, 16),), device=dev, dtype=torch.uint8)
-        N.call('effdet_soft_nms_batch', cls, N.f32(boxes), N.f32(scores), classes.data_ptr(), keys.data_ptr(),
+        N.call('effdet_soft_nms_batch_classes' if per_class else 'effdet_soft_nms_batch', cls, N.f32(boxes), N.f32(scores), classes.data_ptr(), keys.data_ptr(),
                count.data_ptr(), B, A, npad, cap, method, float(iou_threshold), float(sigma), float(threshold),
                ws.data_ptr(), ws_bytes, N.f32(o_s), o_c.data_ptr(), N.f32(o_b), nkeep.data_ptr())
     else:
         _hard_nms(cls, boxes, scores, classes, keys, count, B, A, npad, cap, float(iou_threshold), o_s, o_c, o_b,
-                  nkeep)
+                  nkeep, per_class)
     if not eager:
         return Detections(o_s, o_c, o_b, nkeep)
     m = nkeep.tolist()                               # host read 2 of 2
     return [[o_s[b, :m[b]], o_c[b, :m[b]], o_b[b, :m[b]]] for b in range(B)]
 
 
-def _hard_nms(cls, boxes, scores, classes, keys, count, B, A, npad, cap, iou_threshold, o_s, o_c, o_b, nkeep):
-    """greedy NMS (effdet_nms_batch_chunked) of the sorted candidates, then the gather into the padded outputs"""
+def _hard_nms(cls, boxes, scores, classes, keys, count, B, A, npad, cap, iou_threshold, o_s, o_c, o_b, nkeep,
+              per_class=False):
+    """greedy NMS (effdet_nms_batch_chunked, or effdet_nms_batch_chunked_classes per class) of the sorted candidates,
+    then the gather into the padded outputs"""
     dev = cls.device
     chunk = min(cap, NMS_CHUNK)
     per_image = _nms_workspace(1, cap, chunk)
@@ -1196,8 +1247,13 @@ def _hard_nms(cls, boxes, scores, classes, keys, count, B, A, npad, cap, iou_thr
     ws = torch.empty((ws_bytes // 8,), device=dev, dtype=torch.int64)
     keep = torch.empty((B, cap), device=dev, dtype=torch.int32)
     for b0 in range(0, B, group):
-        N.call('effdet_nms_batch_chunked', cls, N.f32(boxes[b0:]), keys[b0:].data_ptr(), count[b0:].data_ptr(),
-               min(group, B - b0), A, npad, cap, chunk, iou_threshold, ws.data_ptr(), ws_bytes,
-               keep[b0:].data_ptr(), nkeep[b0:].data_ptr())
+        if per_class:
+            N.call('effdet_nms_batch_chunked_classes', cls, N.f32(boxes[b0:]), keys[b0:].data_ptr(),
+                   count[b0:].data_ptr(), classes[b0:].data_ptr(), min(group, B - b0), A, npad, cap, chunk,
+                   iou_threshold, ws.data_ptr(), ws_bytes, keep[b0:].data_ptr(), nkeep[b0:].data_ptr())
+        else:
+            N.call('effdet_nms_batch_chunked', cls, N.f32(boxes[b0:]), keys[b0:].data_ptr(), count[b0:].data_ptr(),
+                   min(group, B - b0), A, npad, cap, chunk, iou_threshold, ws.data_ptr(), ws_bytes,
+                   keep[b0:].data_ptr(), nkeep[b0:].data_ptr())
     N.call('effdet_gather_detections_batch', cls, N.f32(boxes), N.f32(scores), classes.data_ptr(), keep.data_ptr(),
            nkeep.data_ptr(), B, A, cap, N.f32(o_s), o_c.data_ptr(), N.f32(o_b))

@@ -9,7 +9,10 @@ around sm_90a kernels.  Same constructor, attributes, call convention and state-
 Post-processing follows the attributes threshold, iou_threshold, nms and soft_nms_sigma, which may be set after
 construction: nms='hard' (default) is the reference's torchvision NMS; 'linear' and 'gaussian' are Soft-NMS
 (Bodla et al., ICCV 2017), which decays the scores of overlapping boxes instead of dropping them and returns the
-decayed scores.
+decayed scores.  class_nms and pre_nms_top_k choose which boxes may suppress each other: 'agnostic' (default) is the
+reference's one label per anchor and NMS across classes; 'per_class' suppresses only within a class; 'multi_label'
+makes every (anchor, class) pair above the threshold a candidate, keeps the best pre_nms_top_k of them and runs
+per-class NMS on those.
 
 What differs underneath: features stay NHWC end to end, the head writes the level-concatenated
 ``[B, sum(HWA), K]`` / ``[B, sum(HWA), 4]`` tensors directly (no ``torch.cat``), anchors are cached per input
@@ -46,12 +49,14 @@ def _reference_reinit(model):
 
 class EfficientDet(nn.Module):
     def __init__(self, num_classes, network='efficientdet-d0', D_bifpn=3, W_bifpn=88, D_class=3, is_training=True,
-                 threshold=0.01, iou_threshold=0.5, nms='hard', soft_nms_sigma=0.5):
+                 threshold=0.01, iou_threshold=0.5, nms='hard', soft_nms_sigma=0.5, class_nms='agnostic',
+                 pre_nms_top_k=5000):
         super().__init__()
         # D_class is accepted and ignored, as in the reference (the head depth is fixed at 4 convs)
         self.is_training = is_training
         self.threshold, self.iou_threshold = threshold, iou_threshold
         self.nms, self.soft_nms_sigma = nms, soft_nms_sigma
+        self.class_nms, self.pre_nms_top_k = class_nms, pre_nms_top_k
         self.postprocess()
         # registration order backbone -> neck -> bbox_head fixes the state-dict order
         self.backbone = EfficientNet.from_pretrained(MODEL_MAP[network])
@@ -98,12 +103,21 @@ class EfficientDet(nn.Module):
         return self.criterion(cls, reg, anchors, annotations, counts)
 
     def postprocess(self):
-        """the post-processing settings as _ops.detect_batch's keyword arguments (threshold, iou_threshold, nms, sigma),
-        checked: an unknown nms, a soft_nms_sigma that is not finite and > 0, or a linear iou_threshold outside [0, 1]
-        raises EffdetNativeError"""
+        """the post-processing settings as _ops.detect_batch's keyword arguments (threshold, iou_threshold, nms, sigma,
+        class_nms, pre_nms_top_k), checked: an unknown nms or class_nms, a soft_nms_sigma that is not finite and > 0, a
+        linear iou_threshold outside [0, 1] or a pre_nms_top_k that is not an int >= 1 raises EffdetNativeError.
+        class_nms and pre_nms_top_k are left out while both are at their defaults ('agnostic', 5000), which are
+        detect_batch's too: the dict of a model at the defaults stays the four-key dict of earlier versions, and any
+        change to either still changes the dict.  A model that borrows this method without the two attributes gets
+        the defaults."""
         _ops.nms_method(self.nms, self.soft_nms_sigma, self.iou_threshold)
-        return dict(threshold=self.threshold, iou_threshold=self.iou_threshold, nms=self.nms,
+        class_nms, top_k = getattr(self, 'class_nms', 'agnostic'), getattr(self, 'pre_nms_top_k', 5000)
+        _ops.check_class_nms(class_nms, top_k)
+        post = dict(threshold=self.threshold, iou_threshold=self.iou_threshold, nms=self.nms,
                     sigma=self.soft_nms_sigma)
+        if (class_nms, top_k) != ('agnostic', 5000):
+            post.update(class_nms=class_nms, pre_nms_top_k=top_k)
+        return post
 
     def _detections(self, image):
         post = self.postprocess()

@@ -439,7 +439,9 @@ def evaluate_coco(dataset, model, threshold=0.05, batch_size=16, max_records=Non
     ({set_name}_bbox_results.json) and summary, with COCOeval's evaluation run on the device (no pycocotools needed).
     Returns COCOeval's 12 stats (None when there are no detections, as the reference returns early); the model is set
     back to training mode at the end, as the reference does.  collater=pipeline.RawCollater(): the dataset yields
-    decoded samples and the Resizer chain runs on the device, as in evaluate()."""
+    decoded samples and the Resizer chain runs on the device, as in evaluate().  max_records (default 1000 per image)
+    bounds the records above threshold; with model.class_nms = 'multi_label' an image can have more than 1000, and then
+    the refusal names the max_records that would fit."""
     _refuse_training(model, 'evaluate_coco')
     dev = next(model.parameters()).device
     acc = COCOAccumulator(dataset.coco, dataset.image_ids, dataset.label_to_coco_label, score_threshold=threshold,

@@ -330,8 +330,9 @@ class GraphedDetect:
     decoded anchors and their sort keys (24 bytes per anchor plus 8 per power-of-two padded anchor) do not depend on C.
 
     The packed weights and folded BatchNorm are derived inside the graph, so replays follow in-place weight updates
-    (load_state_dict, EMA copies).  The post-processing settings (threshold, iou_threshold, nms, soft_nms_sigma) are
-    fixed at capture: changing one on the model makes the next call raise."""
+    (load_state_dict, EMA copies).  The post-processing settings (threshold, iou_threshold, nms, soft_nms_sigma,
+    class_nms, pre_nms_top_k) are fixed at capture: changing one on the model makes the next call raise.  With
+    class_nms='multi_label', C is also clamped to the min(pre_nms_top_k, A*K) candidate slots of an image."""
 
     _capture_error_mode = 'global'
 

@@ -410,6 +410,39 @@ int effdet_soft_nms_batch(const float* boxes, const float* scores, const int32_t
                           double sigma, float threshold, void* workspace, int64_t workspace_bytes, float* out_scores,
                           int64_t* out_classes, float* out_boxes, int32_t* out_count, int device,
                           effdet_stream_t stream);
+/* Class-aware NMS.  Per-class greedy NMS: effdet_nms_batch_chunked's arguments and workspace plus classes [B,A] int32
+ * (as effdet_detect_candidates_batch writes them); a pair of candidates counts only when their classes are equal.  The
+ * candidates of one class, taken in the global (score desc, anchor asc) order, are that class's own sorted list, so
+ * keep_idx holds torchvision's per-class keep sets (_batched_nms_vanilla) merged in (score desc, anchor asc) order. */
+int effdet_nms_batch_chunked_classes(const float* boxes, const uint64_t* keys, const int32_t* count,
+                                     const int32_t* classes, int B, int A, int npad, int cap, int chunk,
+                                     double iou_threshold, void* workspace, int64_t workspace_bytes, int32_t* keep_idx,
+                                     int32_t* nkeep, int device, effdet_stream_t stream);
+/* Per-class Soft-NMS: effdet_soft_nms_batch's arguments, refusals and workspace.  Picks go in the global order; a pick
+ * decays only the live candidates of its own class (classes [B,A]), the others stay live and unchanged. */
+int effdet_soft_nms_batch_classes(const float* boxes, const float* scores, const int32_t* classes,
+                                  const uint64_t* keys, const int32_t* count, int B, int A, int npad, int cap,
+                                  int method, double iou_threshold, double sigma, float threshold, void* workspace,
+                                  int64_t workspace_bytes, float* out_scores, int64_t* out_classes, float* out_boxes,
+                                  int32_t* out_count, int device, effdet_stream_t stream);
+/* Multi-label candidates: every (anchor a, class k) pair with cls[b,a,k] > threshold, numbered p = a*K + k, and the
+ * best k' = min(top_k, A*K) of them in (score desc, p asc) order, selected exactly by a radix select on the unique
+ * 64-bit key (~order(score) << 32) | p.  Written in effdet_detect_candidates_batch's format with the k' slots in place
+ * of the anchors, so the NMS entries run on it with A := k' and npad := kpad:
+ *   boxes [B,k',4] (16-byte aligned): slot i's pair's anchor box, decoded and clipped bit for bit as the candidates
+ *        entry decodes it; scores [B,k'] its cls value; classes [B,k'] int32 its k; slots >= count[b] are zero
+ *   keys [B,kpad] (kpad = pow2 >= k'): (~order(score) << 32) | slot, sorted; ~0 sentinels from count[b] on
+ *   count [B] int32: min(pairs above threshold, k')
+ *   1 <= B <= 65535, A*K < 2^32, top_k >= 1; cls [B,A,K], reg [B,A,4] and anchors [A,4] as for the candidates entry
+ *   workspace: effdet_detect_topk_workspace(B, A, K, top_k) bytes, 16-byte aligned (-1 when the arguments are refused)
+ * The launch sequence depends on B, A, K and top_k only and there is no host read (capturable).  cls is read once per
+ * histogram pass an image still takes part in (one to six; one when it has at most k' pairs above the threshold) and
+ * once by the compaction. */
+int64_t effdet_detect_topk_workspace(int B, int A, int K, int top_k);
+int effdet_detect_topk_batch(const float* cls, const float* reg, const float* anchors, int B, int A, int K, float img_w,
+                             float img_h, float threshold, int top_k, int kpad, void* workspace,
+                             int64_t workspace_bytes, float* boxes, float* scores, int32_t* classes, uint64_t* keys,
+                             int32_t* count, int device, effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) rank 1: the optimizer step that follows backward in the reference loop,
