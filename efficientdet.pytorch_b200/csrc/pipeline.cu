@@ -53,11 +53,14 @@ __global__ void __launch_bounds__(256) normalize_pad_kernel(const uint8_t* __res
 // The input of the Normalizer is float32(u8) (COCO) or float32(u8) / 255.f (VOC, datasets/voc0712.py:109); since it
 // only depends on the byte, each block first tabulates the 3 x 256 normalized float64 values in shared memory.
 // One thread per output pixel (x fastest); each reads at most 4 source pixels, whose bytes stay in L1/L2.
-__global__ void __launch_bounds__(256) resize_normalize_pad_kernel(const uint8_t* __restrict__ pix, const int64_t* __restrict__ offs,
-                                                                   const int32_t* __restrict__ hw, const int32_t* __restrict__ rhw,
-                                                                   const uint8_t* __restrict__ flip, float* __restrict__ out, int S,
-                                                                   int div255, double m0, double m1, double m2, double s0,
-                                                                   double s1, double s2) {
+// kCrop (scale jitter): output pixel (y, x) is pixel (y + y0, x + x0) of the resized image, (y0, x0) = crops[b], and 0
+// where that lies outside it (the window past the resized image, or a negative offset).  Without kCrop, y0 = x0 = 0.
+template <bool kCrop>
+__device__ __forceinline__ void resize_normalize_pad_body(const uint8_t* __restrict__ pix, const int64_t* __restrict__ offs,
+                                                          const int32_t* __restrict__ hw, const int32_t* __restrict__ rhw,
+                                                          const int32_t* __restrict__ crops, const uint8_t* __restrict__ flip,
+                                                          float* __restrict__ out, int S, int div255, double m0, double m1,
+                                                          double m2, double s0, double s1, double s2) {
     __shared__ double lut[3][256];
     const int b = blockIdx.z;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
@@ -65,7 +68,9 @@ __global__ void __launch_bounds__(256) resize_normalize_pad_kernel(const uint8_t
     const int h = hw[2 * b], w = hw[2 * b + 1], rh = rhw[2 * b], rw = rhw[2 * b + 1];
     const long long plane = (long long)S * S;
     float* o = out + (long long)b * 3 * plane + (long long)y * S + x;
-    if (y >= rh || h <= 0 || w <= 0) {                                  // block-uniform: a padding row
+    const int y0 = kCrop ? crops[2 * b] : 0, x0 = kCrop ? crops[2 * b + 1] : 0;
+    const int Y = y + y0;                                               // the row of the resized image
+    if (Y >= rh || h <= 0 || w <= 0 || (kCrop && (y0 < 0 || x0 < 0))) { // block-uniform: a padding row
         if (x < S) o[0] = o[plane] = o[2 * plane] = 0.f;
         return;
     }
@@ -78,8 +83,9 @@ __global__ void __launch_bounds__(256) resize_normalize_pad_kernel(const uint8_t
     }
     __syncthreads();
     if (x >= S) return;
+    const int X = x + x0;                                               // the column of the resized image
     double v[3] = {0.0, 0.0, 0.0};                                      // np.zeros((S, S, 3)) padding
-    if (x < rw) {
+    if (X < rw) {
         const uint8_t* img = pix + offs[b];
         const bool fl = flip && flip[b];
         // source pixel (r, c) of the flipped image: image[:, ::-1, :]
@@ -87,22 +93,22 @@ __global__ void __launch_bounds__(256) resize_normalize_pad_kernel(const uint8_t
         const double scale_x = __ddiv_rn(1.0, __ddiv_rn((double)rw, (double)w));
         const double scale_y = __ddiv_rn(1.0, __ddiv_rn((double)rh, (double)h));
         if (rh == h && rw == w) {
-            const uint8_t* p = px(y, x);
+            const uint8_t* p = px(Y, X);
             for (int c = 0; c < 3; ++c) v[c] = lut[c][p[c]];
         } else if (fabs(__dsub_rn(scale_x, 2.0)) < DBL_EPSILON && fabs(__dsub_rn(scale_y, 2.0)) < DBL_EPSILON) {
-            const uint8_t *p00 = px(2 * y, 2 * x), *p01 = px(2 * y, 2 * x + 1);
-            const uint8_t *p10 = px(2 * y + 1, 2 * x), *p11 = px(2 * y + 1, 2 * x + 1);
+            const uint8_t *p00 = px(2 * Y, 2 * X), *p01 = px(2 * Y, 2 * X + 1);
+            const uint8_t *p10 = px(2 * Y + 1, 2 * X), *p11 = px(2 * Y + 1, 2 * X + 1);
             for (int c = 0; c < 3; ++c)
                 v[c] = __dmul_rn(__dadd_rn(__dadd_rn(__dadd_rn(lut[c][p00[c]], lut[c][p01[c]]), lut[c][p10[c]]), lut[c][p11[c]]),
                                  0.25);
         } else {
-            float fx = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)x, 0.5), scale_x), 0.5));
+            float fx = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)X, 0.5), scale_x), 0.5));
             int sx = (int)floorf(fx);
             fx = __fsub_rn(fx, (float)sx);
             if (sx < 0) fx = 0.f, sx = 0;
             const bool single = sx + 1 >= w;
             if (sx >= w - 1) fx = 0.f, sx = w - 1;
-            float fy = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)y, 0.5), scale_y), 0.5));
+            float fy = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)Y, 0.5), scale_y), 0.5));
             const int sy = (int)floorf(fy);
             fy = __fsub_rn(fy, (float)sy);
             const int r0 = min(max(sy, 0), h - 1), r1 = min(max(sy + 1, 0), h - 1);
@@ -120,6 +126,27 @@ __global__ void __launch_bounds__(256) resize_normalize_pad_kernel(const uint8_t
     o[0] = (float)v[0];                                                 // the .float() of train.py:105
     o[plane] = (float)v[1];
     o[2 * plane] = (float)v[2];
+}
+
+__global__ void __launch_bounds__(256) resize_normalize_pad_kernel(const uint8_t* __restrict__ pix, const int64_t* __restrict__ offs,
+                                                                   const int32_t* __restrict__ hw, const int32_t* __restrict__ rhw,
+                                                                   const uint8_t* __restrict__ flip, float* __restrict__ out, int S,
+                                                                   int div255, double m0, double m1, double m2, double s0,
+                                                                   double s1, double s2) {
+    resize_normalize_pad_body<false>(pix, offs, hw, rhw, nullptr, flip, out, S, div255, m0, m1, m2, s0, s1, s2);
+}
+
+// Scale jitter: the S x S window at crops[b] = (y0, x0) of the image resized to resized_hw[b] (Resizer at the drawn
+// common size L), zero where the window runs past it.
+__global__ void __launch_bounds__(256) resize_crop_normalize_pad_kernel(const uint8_t* __restrict__ pix,
+                                                                        const int64_t* __restrict__ offs,
+                                                                        const int32_t* __restrict__ hw,
+                                                                        const int32_t* __restrict__ rhw,
+                                                                        const int32_t* __restrict__ crops,
+                                                                        const uint8_t* __restrict__ flip,
+                                                                        float* __restrict__ out, int S, int div255, double m0,
+                                                                        double m1, double m2, double s0, double s1, double s2) {
+    resize_normalize_pad_body<true>(pix, offs, hw, rhw, crops, flip, out, S, div255, m0, m1, m2, s0, s1, s2);
 }
 
 // demo.py's test transform, get_augumentation(phase='test') (datasets/augmentation.py:38-48, albumentations 0.5.2):
@@ -252,13 +279,15 @@ __global__ void collate_annots_kernel(const double* __restrict__ rows, const int
 // kept unless its float32 label is -1, in order, into the front of slot b of out [Bcap,Gcap,5], -1 rows after them.
 // counts[1+b] = rows kept (0 for b >= B), counts[0] = B.  One CTA per slot b < Bcap; every image has <= Gcap rows (the
 // host checks it).
-__global__ void __launch_bounds__(256) collate_pack_annots_kernel(const int64_t* __restrict__ header,
-                                                                  const double* __restrict__ rows,
-                                                                  const int32_t* __restrict__ row_off,
-                                                                  const double* __restrict__ scale,
-                                                                  const uint8_t* __restrict__ flip,
-                                                                  const int32_t* __restrict__ hw, float* __restrict__ out,
-                                                                  int32_t* __restrict__ counts, int Gcap) {
+// kCrop (scale jitter): after the scale, x1/x2 -= x0 and y1/y2 -= y0 ((y0, x0) = crops[b]), each coordinate clamped to
+// [0, S] (S = header[4]), all in float64, then the one cast to float32; a row is kept only if, in float32, its label is
+// not -1, x2 > x1 and y2 > y1.  A NaN coordinate stays NaN through the clamp, so its row is dropped.
+template <bool kCrop>
+__device__ __forceinline__ void collate_pack_annots_body(const int64_t* __restrict__ header, const double* __restrict__ rows,
+                                                         const int32_t* __restrict__ row_off, const double* __restrict__ scale,
+                                                         const uint8_t* __restrict__ flip, const int32_t* __restrict__ hw,
+                                                         const int32_t* __restrict__ crops, float* __restrict__ out,
+                                                         int32_t* __restrict__ counts, int Gcap) {
     __shared__ int warp_tot[32];
     const int b = blockIdx.x;
     const int B = (int)header[0];
@@ -268,6 +297,12 @@ __global__ void __launch_bounds__(256) collate_pack_annots_kernel(const int64_t*
         const int r_begin = row_off[b], n = row_off[b + 1] - r_begin;
         const bool fl = flip[b] != 0;
         const double cols = (double)hw[2 * b + 1], sc = scale[b];
+        const double y0 = kCrop ? (double)crops[2 * b] : 0.0, x0 = kCrop ? (double)crops[2 * b + 1] : 0.0;
+        const double S = kCrop ? (double)header[4] : 0.0;
+        auto crop = [&](double v, double o) {                           // v - o, clamped to [0, S] (NaN passes)
+            const double c = __dsub_rn(v, o);
+            return c < 0.0 ? 0.0 : (c > S ? S : c);
+        };
         for (int g0 = 0; g0 < n; g0 += blockDim.x) {                    // CTA-uniform trip count
             const int g = g0 + threadIdx.x;
             float v[5];
@@ -280,12 +315,19 @@ __global__ void __launch_bounds__(256) collate_pack_annots_kernel(const int64_t*
                     x1 = nx1;
                     x2 = nx2;
                 }
-                v[0] = (float)__dmul_rn(x1, sc);                        // annots[:, :4] *= scale, then the float32 table
-                v[1] = (float)__dmul_rn(r[1], sc);
-                v[2] = (float)__dmul_rn(x2, sc);
-                v[3] = (float)__dmul_rn(r[3], sc);
+                if (kCrop) {
+                    v[0] = (float)crop(__dmul_rn(x1, sc), x0);
+                    v[1] = (float)crop(__dmul_rn(r[1], sc), y0);
+                    v[2] = (float)crop(__dmul_rn(x2, sc), x0);
+                    v[3] = (float)crop(__dmul_rn(r[3], sc), y0);
+                } else {
+                    v[0] = (float)__dmul_rn(x1, sc);                    // annots[:, :4] *= scale, then the float32 table
+                    v[1] = (float)__dmul_rn(r[1], sc);
+                    v[2] = (float)__dmul_rn(x2, sc);
+                    v[3] = (float)__dmul_rn(r[3], sc);
+                }
                 v[4] = (float)r[4];
-                keep = v[4] != -1.f;
+                keep = v[4] != -1.f && (!kCrop || (v[2] > v[0] && v[3] > v[1]));
             }
             int total;
             const int incl = block_scan(keep ? 1 : 0, warp_tot, IntAdd(), total);
@@ -302,6 +344,28 @@ __global__ void __launch_bounds__(256) collate_pack_annots_kernel(const int64_t*
         counts[1 + b] = kept;
         if (b == 0) counts[0] = B;
     }
+}
+
+__global__ void __launch_bounds__(256) collate_pack_annots_kernel(const int64_t* __restrict__ header,
+                                                                  const double* __restrict__ rows,
+                                                                  const int32_t* __restrict__ row_off,
+                                                                  const double* __restrict__ scale,
+                                                                  const uint8_t* __restrict__ flip,
+                                                                  const int32_t* __restrict__ hw, float* __restrict__ out,
+                                                                  int32_t* __restrict__ counts, int Gcap) {
+    collate_pack_annots_body<false>(header, rows, row_off, scale, flip, hw, nullptr, out, counts, Gcap);
+}
+
+__global__ void __launch_bounds__(256) collate_pack_annots_crop_kernel(const int64_t* __restrict__ header,
+                                                                       const double* __restrict__ rows,
+                                                                       const int32_t* __restrict__ row_off,
+                                                                       const double* __restrict__ scale,
+                                                                       const uint8_t* __restrict__ flip,
+                                                                       const int32_t* __restrict__ hw,
+                                                                       const int32_t* __restrict__ crops,
+                                                                       float* __restrict__ out, int32_t* __restrict__ counts,
+                                                                       int Gcap) {
+    collate_pack_annots_body<true>(header, rows, row_off, scale, flip, hw, crops, out, counts, Gcap);
 }
 
 }  // namespace effdet
@@ -334,6 +398,23 @@ extern "C" int effdet_resize_normalize_pad(const uint8_t* pixels, const int64_t*
                                                                        pixel_scale == 255, mean3[0], mean3[1], mean3[2],
                                                                        std3[0], std3[1], std3[2]);
     return launch_status("resize_normalize_pad_kernel");
+}
+
+extern "C" int effdet_resize_crop_normalize_pad(const uint8_t* pixels, const int64_t* offsets, const int32_t* hw,
+                                                const int32_t* resized_hw, const int32_t* crops, const uint8_t* flip,
+                                                float* out_nchw, int B, int S, int pixel_scale, const double* mean3,
+                                                const double* std3, int device, effdet_stream_t stream) {
+    EFFDET_REQUIRE(pixels && offsets && hw && resized_hw && crops && out_nchw && mean3 && std3 && B > 0 && B <= 65535 &&
+                       S > 0 && S <= 65535,
+                   "resize_crop_normalize_pad: bad arguments");
+    EFFDET_REQUIRE(pixel_scale == 1 || pixel_scale == 255, "resize_crop_normalize_pad: pixel_scale %d not in {1,255}",
+                   pixel_scale);
+    EFFDET_DEVICE(device);
+    dim3 grid(cdiv(S, 256), S, B);
+    resize_crop_normalize_pad_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(pixels, offsets, hw, resized_hw, crops, flip,
+                                                                            out_nchw, S, pixel_scale == 255, mean3[0],
+                                                                            mean3[1], mean3[2], std3[0], std3[1], std3[2]);
+    return launch_status("resize_crop_normalize_pad_kernel");
 }
 
 extern "C" int effdet_frame_transform(const uint8_t* pixels, const int64_t* offsets, const int32_t* hw, float* out_nchw, int B,
@@ -381,4 +462,19 @@ extern "C" int effdet_collate_pack_annots(const int64_t* header, const double* r
     collate_pack_annots_kernel<<<Bcap, 256, 0, (cudaStream_t)stream>>>(header, rows, row_off, scale, flip, hw, out, counts,
                                                                       Gcap);
     return launch_status("collate_pack_annots_kernel");
+}
+
+extern "C" int effdet_collate_pack_annots_crop(const int64_t* header, const double* rows, const int32_t* row_off,
+                                               const double* scale, const uint8_t* flip, const int32_t* hw,
+                                               const int32_t* crops, float* out, int32_t* counts, int Bcap, int Gcap,
+                                               int device, effdet_stream_t stream) {
+    EFFDET_REQUIRE(header && rows && row_off && scale && flip && hw && crops && out && counts,
+                   "collate_pack_annots_crop: null argument");
+    EFFDET_REQUIRE(Bcap > 0 && Bcap <= 65535 && Gcap > 0 && Gcap <= INT_MAX / 5,
+                   "collate_pack_annots_crop: capacity Bcap=%d, Gcap=%d unsupported (1..65535, 1..%d)", Bcap, Gcap,
+                   INT_MAX / 5);
+    EFFDET_DEVICE(device);
+    collate_pack_annots_crop_kernel<<<Bcap, 256, 0, (cudaStream_t)stream>>>(header, rows, row_off, scale, flip, hw, crops,
+                                                                           out, counts, Gcap);
+    return launch_status("collate_pack_annots_crop_kernel");
 }

@@ -174,6 +174,8 @@ SIGNATURES = {
     'effdet_resize_normalize_pad': [_P] * 6 + [_INT] * 3 + [ctypes.POINTER(ctypes.c_double)] * 2 + _TAIL,
     'effdet_collate_annots': [_P, _P, _P, _P, _P, _P, _INT, _INT] + _TAIL,
     'effdet_collate_pack_annots': [_P] * 8 + [_INT, _INT] + _TAIL,
+    'effdet_resize_crop_normalize_pad': [_P] * 7 + [_INT] * 3 + [ctypes.POINTER(ctypes.c_double)] * 2 + _TAIL,
+    'effdet_collate_pack_annots_crop': [_P] * 9 + [_INT, _INT] + _TAIL,
     'effdet_frame_transform': [_P] * 4 + [_INT] * 3 + [ctypes.POINTER(ctypes.c_float)] * 2 + _TAIL,
     'effdet_frame_boxes': [_P] * 5 + [_INT] * 4 + [_P, _P] + _TAIL,
     'effdet_eval_select': [_P, _P, _P, _INT, _F, _F, _INT, _INT, _P, _P, _P, _P] + _TAIL,

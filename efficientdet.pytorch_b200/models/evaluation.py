@@ -203,6 +203,12 @@ def _detect_all(dataset, model, acc, batch_size, per_image, progress_base, colla
                 print('{}/{}'.format(i + progress_base, n), end='\r')
 
 
+def _refuse_jitter(collater, what):
+    if getattr(collater, 'scale_jitter', None) is not None:
+        raise N.EffdetNativeError('%s: the collater has scale_jitter=%r, but evaluation never jitters; pass a '
+                                  'RawCollater without scale_jitter' % (what, collater.scale_jitter))
+
+
 def _refuse_training(model, what):
     if model.training or model.is_training:
         raise N.EffdetNativeError('%s needs a model in inference mode (model.eval() and model.is_training = False)'
@@ -219,7 +225,9 @@ def evaluate(generator, retinanet, iou_threshold=0.5, score_threshold=0.05, max_
     collater=pipeline.RawCollater(pixel_scale=255): `generator[i]` yields decoded samples ({'img': uint8 [h,w,3],
     'annot'}, as DeviceCollater takes them) instead; a DataLoader(generator, batch_size, num_workers=num_workers,
     collate_fn=collater, pin_memory=True) batches them and the Resizer chain runs on the device, bit-identical to the
-    host chain, inside a GraphedRawDetect.  Ground truth still comes from generator.load_annotations."""
+    host chain, inside a GraphedRawDetect.  Ground truth still comes from generator.load_annotations.  A collater with
+    scale_jitter is refused."""
+    _refuse_jitter(collater, 'evaluate')
     _refuse_training(retinanet, 'evaluate')
     n, K = len(generator), generator.num_classes()
     dev = next(retinanet.parameters()).device
@@ -441,7 +449,8 @@ def evaluate_coco(dataset, model, threshold=0.05, batch_size=16, max_records=Non
     back to training mode at the end, as the reference does.  collater=pipeline.RawCollater(): the dataset yields
     decoded samples and the Resizer chain runs on the device, as in evaluate().  max_records (default 1000 per image)
     bounds the records above threshold; with model.class_nms = 'multi_label' an image can have more than 1000, and then
-    the refusal names the max_records that would fit."""
+    the refusal names the max_records that would fit.  A collater with scale_jitter is refused."""
+    _refuse_jitter(collater, 'evaluate_coco')
     _refuse_training(model, 'evaluate_coco')
     dev = next(model.parameters()).device
     acc = COCOAccumulator(dataset.coco, dataset.image_ids, dataset.label_to_coco_label, score_threshold=threshold,

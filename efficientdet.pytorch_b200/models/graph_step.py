@@ -51,6 +51,11 @@ is copied.
         step = step or GraphedTrainStep(model, raw, optimizer=opt, max_annotations=256)
         loss = step(raw, update=(idx + 1) % k == 0)
 
+With RawCollater(..., scale_jitter=(lo, hi)) the batches are scale-jittered (RawBatch.jitter): a step built on one
+captures the crop variants of the two launches (effdet_resize_crop_normalize_pad, effdet_collate_pack_annots_crop),
+and every replay takes the new batch's drawn sizes and windows from its blob.  A step captured for jittered batches
+refuses unjittered ones, and the reverse.
+
 Training with the optimizer in the graph.  With `optimizer=FusedClipAdamW(...)` every call is one micro-step of the
 reference loop (train.py:95-133): forward, loss, backward, gradients added to the persistent accumulators that
 `p.grad` then refers to (skipped when the loss is exactly 0), and, when `update` is true and the loss is non-zero, the
@@ -182,9 +187,10 @@ class GraphedTrainStep:
             raise err('GraphedTrainStep needs a model on a CUDA device')
         Bcap = example.B
         cap_bytes = Bcap * int(example.image_bytes.max()) if max_bytes is None else int(max_bytes)
-        _, total = pipeline.raw_layout(Bcap, Bcap * max_annotations, cap_bytes)
+        _, total = pipeline.raw_layout(Bcap, Bcap * max_annotations, cap_bytes, example.jitter)
         self.raw = dict(Bcap=Bcap, Gcap=max_annotations, max_bytes=cap_bytes, S=example.S,
-                        pixel_scale=example.pixel_scale, blob=torch.empty((total,), dtype=torch.uint8, device=dev))
+                        pixel_scale=example.pixel_scale, jitter=example.jitter,
+                        blob=torch.empty((total,), dtype=torch.uint8, device=dev))
         self._check_raw(example)
         self._load_raw(example)
         return torch.zeros((Bcap, 3, example.S, example.S), device=dev)
@@ -194,6 +200,10 @@ class GraphedTrainStep:
         err, c = _ops.N.EffdetNativeError, self.raw
         if not isinstance(raw, pipeline.RawBatch):
             raise err('GraphedTrainStep was built on a RawBatch: call it as step(raw_batch, update=...)')
+        if raw.jitter != c['jitter']:
+            kind = ('unjittered', 'scale-jittered')
+            raise err('GraphedTrainStep was captured for %s raw batches, got a batch that is %s; rebuild the step on a '
+                      'batch from the collater you train with' % (kind[c['jitter']], kind[raw.jitter]))
         if (raw.S, raw.pixel_scale) != (c['S'], c['pixel_scale']):
             raise err('GraphedTrainStep was captured for common size %d and pixel_scale %r, got %d and %r'
                       % (c['S'], c['pixel_scale'], raw.S, raw.pixel_scale))
@@ -217,8 +227,8 @@ class GraphedTrainStep:
         """the head of the captured region in raw-batch mode: Normalizer -> flip -> Resizer -> pad into the static
         images (padding images are zeros), then the annotations collated and packed with their counts"""
         c = self.raw
-        pipeline.launch_raw_resize(self.static_images, c['blob'], c['Bcap'], c['pixel_scale'])
-        pipeline.launch_raw_pack(c['blob'], c['Bcap'], self.static_annots, self.static_counts)
+        pipeline.launch_raw_resize(self.static_images, c['blob'], c['Bcap'], c['pixel_scale'], c['jitter'])
+        pipeline.launch_raw_pack(c['blob'], c['Bcap'], self.static_annots, self.static_counts, c['jitter'])
 
     def _eager_step(self, params, zero=True, capture=False):
         if zero:
@@ -526,6 +536,9 @@ class GraphedRawDetect(GraphedDetect):
         err = _ops.N.EffdetNativeError
         if not isinstance(raw, pipeline.RawBatch):
             raise err('GraphedRawDetect takes RawBatch inputs (pipeline.RawCollater output)')
+        if raw.jitter:
+            raise err('GraphedRawDetect takes unjittered raw batches: detection and evaluation never jitter; use a '
+                      'RawCollater without scale_jitter')
         if (raw.S, raw.pixel_scale) != (self.S, self.pixel_scale):
             raise err('GraphedRawDetect was captured for common size %d and pixel_scale %r, got %d and %r'
                       % (self.S, self.pixel_scale, raw.S, raw.pixel_scale))

@@ -13,6 +13,7 @@
                       the network in one CUDA graph.
 """
 import ctypes
+import math
 
 import numpy as np
 import torch
@@ -44,10 +45,12 @@ def concat_pinned(imgs, staging=None):
     return flat, offs
 
 
-def check_samples(samples, S, resize, who, resize_who):
+def check_samples(samples, S, resize, who, resize_who, jitter=False):
     """the sample checks of DeviceCollater and RawCollater -> (C-contiguous uint8 images, sizes int32 [B, 2], box scales
     float64 [B], resized sizes int32 [B, 2]).  Raises before anything is copied; who / resize_who name the caller in the
-    messages (resize_who in the refusal of 'scale', which only the Resizer path makes)."""
+    messages (resize_who in the refusal of 'scale', which only the Resizer path makes).  jitter: each image's common
+    size is drawn afterwards (RawCollater(scale_jitter=...)), so no geometry is computed or refused here and the scales
+    and resized sizes are None."""
     imgs = [np.ascontiguousarray(s['img']) for s in samples]
     for im in imgs:
         if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3 or im.shape[0] < 1 or im.shape[1] < 1 or \
@@ -59,6 +62,8 @@ def check_samples(samples, S, resize, who, resize_who):
         if any('scale' in s for s in samples):
             raise N.EffdetNativeError("%s: a sample carries 'scale', but the Resizer computes each image's scale "
                                       "itself" % resize_who)
+        if jitter:
+            return imgs, sizes, None, None
         geo = [resizer_geometry(int(h), int(w), S) for h, w in sizes]
         for (h, w), (_, rh, rw) in zip(sizes, geo):
             if rh < 1 or rw < 1:
@@ -130,18 +135,20 @@ class DeviceCollater:
 
 
 # ---- raw batches: what DataLoader workers hand to the graphed steps ---------------------------------------------------
-RAW_HEADER = 8          # int64 header entries: B, pixel bytes, rows, layout capacity, common size, pixel scale, 0, 0
+RAW_HEADER = 8          # int64 header entries: B, pixel bytes, rows, layout capacity, common size, pixel scale, jitter, 0
 _MEAN64 = (ctypes.c_double * 3)(*MEAN)
 _STD64 = (ctypes.c_double * 3)(*STD)
 
 
-def raw_layout(capacity, rows, nbytes):
+def raw_layout(capacity, rows, nbytes, jitter=False):
     """byte offset of every section of a raw batch whose per-image sections hold `capacity` images, with `rows`
     annotation rows and `nbytes` pixel bytes -> (dict name -> offset, total bytes).  Every section starts on a 16-byte
-    boundary; the sections up to 'rows' depend on the capacity alone."""
+    boundary; the sections up to 'rows' depend on the capacity (and jitter) alone.  jitter: the batch carries a 'crops'
+    section (int32 [capacity, 2], each image's window offsets (y0, x0)) between 'row_offsets' and 'rows'; the sections
+    before it are where they are without it."""
     sizes = [('header', 8 * RAW_HEADER), ('offsets', 8 * capacity), ('hw', 8 * capacity), ('resized_hw', 8 * capacity),
-             ('flips', capacity), ('scales', 8 * capacity), ('row_offsets', 4 * (capacity + 1)), ('rows', 40 * rows),
-             ('pixels', nbytes)]
+             ('flips', capacity), ('scales', 8 * capacity), ('row_offsets', 4 * (capacity + 1))] + \
+        ([('crops', 8 * capacity)] if jitter else []) + [('rows', 40 * rows), ('pixels', nbytes)]
     off, at = {}, 0
     for name, n in sizes:
         off[name] = at
@@ -151,27 +158,29 @@ def raw_layout(capacity, rows, nbytes):
 
 _SECTIONS = {'header': (torch.int64, RAW_HEADER), 'offsets': (torch.int64, 1), 'hw': (torch.int32, 2),
              'resized_hw': (torch.int32, 2), 'flips': (torch.uint8, 1), 'scales': (torch.float64, 1),
-             'row_offsets': (torch.int32, 1)}
+             'row_offsets': (torch.int32, 1), 'crops': (torch.int32, 2)}
 
 
 def raw_section(blob, capacity, name):
     """a typed view of one fixed section of a raw batch (host or device) laid out for `capacity` images: header int64
     [8], offsets int64 [cap], hw / resized_hw int32 [cap, 2], flips uint8 [cap], scales float64 [cap], row_offsets
-    int32 [cap + 1]"""
-    off, _ = raw_layout(capacity, 0, 0)
+    int32 [cap + 1], crops int32 [cap, 2] (a jittered batch only)"""
+    off, _ = raw_layout(capacity, 0, 0, jitter=True)      # the other fixed sections sit at the same offsets without it
     dtype, width = _SECTIONS[name]
     n = RAW_HEADER if name == 'header' else (capacity + 1 if name == 'row_offsets' else capacity * width)
     v = blob[off[name]:off[name] + n * dtype.itemsize].view(dtype)
     return v.reshape(capacity, width) if width == 2 else v
 
 
-def _assemble(capacity, S, pixel_scale, sizes, resized, flips, scales, counts, rows, pixels, pin=False):
+def _assemble(capacity, S, pixel_scale, sizes, resized, flips, scales, counts, rows, pixels, pin=False, crops=None):
     """one raw batch blob laid out for `capacity` >= B images: entries b >= B of the per-image sections are zero (an
-    image with h = 0 is padding to the resize kernel).  pixels: a list of uint8 arrays, back to back."""
+    image with h = 0 is padding to the resize kernel).  pixels: a list of uint8 arrays, back to back.  crops: int32
+    [B, 2] window offsets of a jittered batch, None otherwise."""
     B = len(sizes)
     image_bytes = sizes[:, 0].astype(np.int64) * sizes[:, 1] * 3
     nbytes, R = int(image_bytes.sum()), int(counts.sum())
-    off, total = raw_layout(capacity, R, nbytes)
+    jitter = crops is not None
+    off, total = raw_layout(capacity, R, nbytes, jitter)
     blob = torch.empty((total,), dtype=torch.uint8, pin_memory=pin)
     a = blob.numpy()
     p0 = off['pixels']
@@ -182,16 +191,18 @@ def _assemble(capacity, S, pixel_scale, sizes, resized, flips, scales, counts, r
         arr = np.ascontiguousarray(arr).reshape(-1).view(np.uint8)
         a[off[name]:off[name] + arr.size] = arr
 
-    put('header', np.array([B, nbytes, R, capacity, S, pixel_scale or 1, 0, 0], np.int64))
+    put('header', np.array([B, nbytes, R, capacity, S, pixel_scale or 1, int(jitter), 0], np.int64))
     put('offsets', p0 + np.concatenate([[0], np.cumsum(image_bytes)[:-1]]).astype(np.int64))   # from the blob's start
     put('hw', sizes.astype(np.int32))
     put('resized_hw', resized.astype(np.int32))
     put('flips', flips.astype(np.uint8))
     put('scales', scales.astype(np.float64))
     put('row_offsets', np.concatenate([[0], np.cumsum(counts)]).astype(np.int32))
+    if jitter:
+        put('crops', crops.astype(np.int32))
     put('rows', rows.astype(np.float64))
     np.concatenate([np.asarray(p).reshape(-1) for p in pixels] or [np.zeros(0, np.uint8)], out=a[p0:p0 + nbytes])
-    return RawBatch(blob, capacity, S, pixel_scale, counts, image_bytes, scales)
+    return RawBatch(blob, capacity, S, pixel_scale, counts, image_bytes, scales, jitter)
 
 
 class RawBatch:
@@ -200,13 +211,16 @@ class RawBatch:
     host-to-device copy.  Sections, each 16-byte aligned (raw_layout): header int64 [8] (B, pixel bytes, rows, layout
     capacity, common size, pixel scale), byte offsets int64 [cap] (from the blob's start), hw and resized_hw int32
     [cap, 2], flips uint8 [cap], Resizer scales float64 [cap], row offsets int32 [cap + 1], rows float64 [R, 5], pixels.
-    A collated batch is laid out for its own B images (capacity == B).
+    A collated batch is laid out for its own B images (capacity == B).  A scale-jittered batch (jitter True, header[6] =
+    1) also has crops int32 [cap, 2] before the rows: the window offsets (y0, x0) of each image, whose resized_hw and
+    scales are then the Resizer's at that image's drawn common size.
 
     Host-side facts, for the capacity checks without a device read: B, counts (rows per image), image_bytes, nbytes,
     and scales (float64 [B], eval.py's data['scale'], as VOCAccumulator.add() takes them)."""
 
-    def __init__(self, blob, capacity, S, pixel_scale, counts, image_bytes, scales):
+    def __init__(self, blob, capacity, S, pixel_scale, counts, image_bytes, scales, jitter=False):
         self.blob = blob
+        self.jitter = bool(jitter)
         self.capacity, self.S, self.pixel_scale = int(capacity), int(S), pixel_scale
         self.counts = np.asarray(counts, dtype=np.int32)
         self.image_bytes = np.asarray(image_bytes, dtype=np.int64)
@@ -232,7 +246,7 @@ class RawBatch:
     def pin_memory(self):
         """a copy in pinned memory (DataLoader(pin_memory=True) calls this in its pin thread)"""
         return RawBatch(self.blob.pin_memory(), self.capacity, self.S, self.pixel_scale, self.counts, self.image_bytes,
-                        self.scales)
+                        self.scales, self.jitter)
 
     def at_capacity(self, capacity, pin=False):
         """the same batch laid out for `capacity` >= B images (zero entries for the unused ones): what a graph captured
@@ -240,12 +254,28 @@ class RawBatch:
         if capacity == self.capacity:
             return self
         B = self.B
-        off, _ = raw_layout(self.capacity, self.rows, self.nbytes)
+        off, _ = raw_layout(self.capacity, self.rows, self.nbytes, self.jitter)
         a = self.blob.numpy()
         rows = a[off['rows']:off['rows'] + 40 * self.rows].view(np.float64).reshape(-1, 5)
         return _assemble(capacity, self.S, self.pixel_scale, self.section('hw')[:B].numpy(),
                          self.section('resized_hw')[:B].numpy(), self.section('flips')[:B].numpy(), self.scales,
-                         self.counts, rows, [a[off['pixels']:off['pixels'] + self.nbytes]], pin=pin)
+                         self.counts, rows, [a[off['pixels']:off['pixels'] + self.nbytes]], pin=pin,
+                         crops=self.section('crops')[:B].numpy() if self.jitter else None)
+
+
+def jitter_range(S, lo, hi):
+    """the common sizes scale_jitter=(lo, hi) draws from at training size S: (L_lo, L_hi), both inclusive"""
+    L_lo = max(1, math.ceil(lo * S))
+    return L_lo, max(L_lo, math.floor(hi * S))
+
+
+def min_common_size(h, w):
+    """the smallest common size L at which resizer_geometry(h, w, L) resizes to at least 1 x 1 (the short side is
+    int(short * (L / long)); it first reaches 1 at L >= long // short)"""
+    L = max(1, max(h, w) // min(h, w) - 1)
+    while min(resizer_geometry(h, w, L)[1:]) < 1:
+        L += 1
+    return L
 
 
 class RawCollater:
@@ -253,48 +283,100 @@ class RawCollater:
     float64 [n,5], optional 'flip'}, no 'scale'), refuses what it refuses, and returns a RawBatch.  It never touches
     CUDA, so it runs in forked workers after the parent has initialised CUDA; GraphedTrainStep / GraphedRawDetect run
     the Normalizer -> Augmenter flip -> Resizer -> collater chain on the device, bit-identical to DeviceCollater.
-    pixel_scale: None (COCO, float32(u8)) or 255 (VOC, float32(u8) / 255), as DeviceCollater."""
+    pixel_scale: None (COCO, float32(u8)) or 255 (VOC, float32(u8) / 255), as DeviceCollater.
 
-    def __init__(self, common_size=512, pixel_scale=None):
+    scale_jitter=(lo, hi), 0 < lo <= hi, both finite: EfficientDet's training augmentation (Tan et al., section 5.1),
+    random scale jittering followed by a crop to S x S.  For each image, in sample order, with NumPy's global
+    np.random (which DataLoader reseeds in every worker), three draws:
+      L = np.random.randint(L_lo, L_hi + 1), L_lo = max(1, ceil(lo * S)), L_hi = max(L_lo, floor(hi * S)); then L is
+        raised to min_common_size(h, w) if below it, so that the Resizer at L never resizes a side to 0;
+      (scale, rh, rw) = resizer_geometry(h, w, L);
+      y0 = np.random.randint(0, max(rh - S, 0) + 1), x0 = np.random.randint(0, max(rw - S, 0) + 1).
+    On the device (GraphedTrainStep), image b is Normalizer -> flip -> Resizer at common size L -> the S x S window at
+    (y0, x0), zero where it runs past the resized image; its boxes are flipped and scaled as without jitter, shifted by
+    (x0, y0) and clamped to [0, S] in float64, and rows with zero area in float32 are dropped.  scale_jitter=(1, 1)
+    gives L = S and (y0, x0) = (0, 0): the unjittered images and boxes.  Evaluation never jitters: evaluate(),
+    evaluate_coco() and GraphedRawDetect refuse such a collater or its batches."""
+
+    def __init__(self, common_size=512, pixel_scale=None, scale_jitter=None):
         if pixel_scale not in (None, 255):
             raise N.EffdetNativeError('RawCollater: pixel_scale must be None (COCO) or 255 (VOC), got %r' % (pixel_scale,))
         self.S, self.pixel_scale = int(common_size), pixel_scale
+        self.scale_jitter = None
+        if scale_jitter is not None:
+            try:
+                lo, hi = (float(v) for v in scale_jitter)
+            except (TypeError, ValueError):
+                lo = hi = float('nan')
+            if not (math.isfinite(lo) and math.isfinite(hi) and 0 < lo <= hi):
+                raise N.EffdetNativeError('RawCollater: scale_jitter must be (lo, hi) with 0 < lo <= hi, both finite, '
+                                          'got %r' % (scale_jitter,))
+            if jitter_range(self.S, lo, hi)[1] > 65535:
+                raise N.EffdetNativeError('RawCollater: scale_jitter=%r draws common sizes up to %d at common size %d; '
+                                          'the most is 65535' % (scale_jitter, jitter_range(self.S, lo, hi)[1], self.S))
+            self.scale_jitter = (lo, hi)
 
     def __call__(self, samples):
-        imgs, sizes, scales, resized = check_samples(samples, self.S, True, 'RawCollater', 'RawCollater')
+        jitter = self.scale_jitter is not None
+        imgs, sizes, scales, resized = check_samples(samples, self.S, True, 'RawCollater', 'RawCollater', jitter)
         flips = np.array([1 if s.get('flip') else 0 for s in samples], dtype=np.uint8)
         anns = [np.asarray(s['annot'], dtype=np.float64).reshape(-1, 5) for s in samples]
         counts = np.array([a.shape[0] for a in anns], dtype=np.int32)
         rows = np.concatenate(anns, axis=0) if counts.sum() else np.zeros((0, 5))
-        return _assemble(len(samples), self.S, self.pixel_scale, sizes, resized, flips, scales, counts, rows, imgs)
+        crops = None
+        if jitter:
+            scales, resized, crops = self._draw(sizes)
+        return _assemble(len(samples), self.S, self.pixel_scale, sizes, resized, flips, scales, counts, rows, imgs,
+                         crops=crops)
+
+    def _draw(self, sizes):
+        """the scale-jitter draws of a batch of images of sizes int32 [B, 2] -> (scales float64 [B], resized sizes
+        int32 [B, 2], window offsets (y0, x0) int32 [B, 2])"""
+        S = self.S
+        L_lo, L_hi = jitter_range(S, *self.scale_jitter)
+        scales, resized, crops = [], [], []
+        for h, w in sizes.tolist():
+            L = max(int(np.random.randint(L_lo, L_hi + 1)), min_common_size(h, w))
+            scale, rh, rw = resizer_geometry(h, w, L)
+            y0 = int(np.random.randint(0, max(rh - S, 0) + 1))
+            x0 = int(np.random.randint(0, max(rw - S, 0) + 1))
+            scales.append(scale)
+            resized.append((rh, rw))
+            crops.append((y0, x0))
+        return (np.array(scales, dtype=np.float64), np.array(resized, dtype=np.int32).reshape(-1, 2),
+                np.array(crops, dtype=np.int32).reshape(-1, 2))
 
 
-def launch_raw_resize(out, blob, capacity, pixel_scale):
+def launch_raw_resize(out, blob, capacity, pixel_scale, jitter=False):
     """effdet_resize_normalize_pad of a raw batch in device memory laid out for `capacity` images into out float32
-    [capacity, 3, S, S]; the geometry arguments point into the blob, and padding entries (h = 0) write zeros"""
+    [capacity, 3, S, S]; the geometry arguments point into the blob, and padding entries (h = 0) write zeros.
+    jitter (RawBatch.jitter, known on the host): effdet_resize_crop_normalize_pad, the window at each image's crops."""
     S = out.shape[2]
     sec = lambda name: raw_section(blob, capacity, name)               # noqa: E731
-    N.call('effdet_resize_normalize_pad', out, N.ptr(blob), N.ptr(sec('offsets')), N.ptr(sec('hw')),
-           N.ptr(sec('resized_hw')), N.ptr(sec('flips')), N.f32(out), capacity, S, pixel_scale or 1, _MEAN64, _STD64,
+    geo = [N.ptr(sec('offsets')), N.ptr(sec('hw')), N.ptr(sec('resized_hw'))] + ([N.ptr(sec('crops'))] if jitter else [])
+    N.call('effdet_resize_crop_normalize_pad' if jitter else 'effdet_resize_normalize_pad', out, N.ptr(blob), *geo,
+           N.ptr(sec('flips')), N.f32(out), capacity, S, pixel_scale or 1, _MEAN64, _STD64,
            nbytes=float(blob.numel() + 4 * out.numel()))
 
 
-def launch_raw_pack(blob, capacity, annots, counts):
+def launch_raw_pack(blob, capacity, annots, counts, jitter=False):
     """effdet_collate_pack_annots of a raw batch in device memory laid out for `capacity` images into the static table
-    annots float32 [capacity, Gcap, 5] and counts int32 [1 + capacity]"""
+    annots float32 [capacity, Gcap, 5] and counts int32 [1 + capacity].  jitter: effdet_collate_pack_annots_crop,
+    the boxes shifted by each image's crops and clamped to the window"""
     sec = lambda name: raw_section(blob, capacity, name)               # noqa: E731
-    rows = blob[raw_layout(capacity, 0, 0)[0]['rows']:]
-    N.call('effdet_collate_pack_annots', annots, N.ptr(sec('header')), N.ptr(rows), N.ptr(sec('row_offsets')),
-           N.ptr(sec('scales')), N.ptr(sec('flips')), N.ptr(sec('hw')), N.f32(annots), N.ptr(counts), capacity,
-           annots.shape[1])
+    rows = blob[raw_layout(capacity, 0, 0, jitter)[0]['rows']:]
+    geo = [N.ptr(sec('hw'))] + ([N.ptr(sec('crops'))] if jitter else [])
+    N.call('effdet_collate_pack_annots_crop' if jitter else 'effdet_collate_pack_annots', annots, N.ptr(sec('header')),
+           N.ptr(rows), N.ptr(sec('row_offsets')), N.ptr(sec('scales')), N.ptr(sec('flips')), *geo, N.f32(annots),
+           N.ptr(counts), capacity, annots.shape[1])
 
 
 def raw_images(raw, device='cuda:0'):
     """the images of a raw batch on the device, eagerly: float32 [B, 3, S, S], bit-identical to DeviceCollater(S,
-    resize=True, pixel_scale=raw.pixel_scale)"""
+    resize=True, pixel_scale=raw.pixel_scale) (a jittered batch: each image's window, as GraphedTrainStep makes it)"""
     blob = raw.blob.to(device, non_blocking=raw.blob.is_pinned())
     out = torch.empty((raw.capacity, 3, raw.S, raw.S), device=blob.device, dtype=torch.float32)
-    launch_raw_resize(out, blob, raw.capacity, raw.pixel_scale)
+    launch_raw_resize(out, blob, raw.capacity, raw.pixel_scale, raw.jitter)
     return out[:raw.B]
 
 

@@ -516,6 +516,21 @@ int effdet_collate_pack_annots(const int64_t* header, const double* rows, const 
 int effdet_resize_normalize_pad(const uint8_t* pixels, const int64_t* offsets, const int32_t* hw, const int32_t* resized_hw,
                                 const uint8_t* flip, float* out_nchw, int B, int S, int pixel_scale, const double* mean3,
                                 const double* std3, int device, effdet_stream_t stream);
+/* Scale jitter (models/pipeline.py RawCollater(scale_jitter=...)): the siblings above plus crops int32 [B,2] (Bcap for
+ * the pack) = (y0, x0) per image.
+ * effdet_resize_crop_normalize_pad: image b is resized to resized_hw[b] (Resizer at the drawn common size L, so up to
+ * L >= S per side) and out[b] is the S x S window at (y0, x0) of it: out[y, x] = R[y + y0, x + x0] where that lies
+ * inside the resized image, 0 elsewhere (a negative offset writes a zero image).
+ * effdet_collate_pack_annots_crop: after the flip and the scale, x1/x2 -= x0 and y1/y2 -= y0, each coordinate clamped
+ * to [0, S] with S = header[4], in float64, then cast to float32 once; a row is kept only if its float32 label is not
+ * -1, x2 > x1 and y2 > y1.  Refusals as the siblings'. */
+int effdet_resize_crop_normalize_pad(const uint8_t* pixels, const int64_t* offsets, const int32_t* hw,
+                                     const int32_t* resized_hw, const int32_t* crops, const uint8_t* flip, float* out_nchw,
+                                     int B, int S, int pixel_scale, const double* mean3, const double* std3, int device,
+                                     effdet_stream_t stream);
+int effdet_collate_pack_annots_crop(const int64_t* header, const double* rows, const int32_t* row_off, const double* scale,
+                                    const uint8_t* flip, const int32_t* hw, const int32_t* crops, float* out,
+                                    int32_t* counts, int Bcap, int Gcap, int device, effdet_stream_t stream);
 /* demo.py's per-frame path (Detect.process, demo.py:71-104) for a batch of frames.
  * effdet_frame_transform replaces get_augumentation(phase='test') + `.to(device).unsqueeze(0)` (demo.py:75-78,
  * datasets/augmentation.py:38-48, albumentations 0.5.2): cv2.resize(frame, (W, H), INTER_LINEAR) of the uint8 frame in
