@@ -141,6 +141,56 @@ __global__ void __launch_bounds__(256) multi_clip_adamw_dev_kernel(
                            bias_c[0], bias_c[1], 0);
 }
 
+// Exponential moving average of the weights (Tan et al. 2020, section 5.1): e = e - w * (e - s) per element, each
+// operation rounded on its own (TF's assign_moving_average: variable - (variable - value) * (1 - decay)), with the
+// decay ramp of TF's ExponentialMovingAverage(decay, num_updates) in fp64 and w = 1 - d rounded once to fp32.  The
+// counter advances once per launch by the last CTA to take a ticket, as in multi_clip_adamw_dev_kernel.
+__global__ void __launch_bounds__(256) multi_ema_kernel(
+    const unsigned long long* __restrict__ ema_ptrs, const unsigned long long* __restrict__ src_ptrs,
+    const long long* __restrict__ numels, const int* __restrict__ chunk_tensor, const long long* __restrict__ chunk_off,
+    int chunk, double decay, int ramp, long long* updates, const int* __restrict__ gate, unsigned int* ticket) {
+    if (gate != nullptr && __ldg(gate) == 0) return;
+    __shared__ float w_s;
+    if (threadIdx.x == 0) {
+        const long long u = *updates;
+        __threadfence();                                       // the read above completes before the ticket
+        if (atomicAdd(ticket, 1u) == gridDim.x - 1) {
+            *ticket = 0u;
+            *updates = u + 1;
+        }
+        const double k = static_cast<double>(u + 1);
+        const double d = ramp ? fmin(decay, (1.0 + k) / (10.0 + k)) : decay;
+        w_s = static_cast<float>(1.0 - d);
+    }
+    __syncthreads();
+    const float w = w_s;
+    const int t = chunk_tensor[blockIdx.x];
+    const long long off = chunk_off[blockIdx.x];
+    float* __restrict__ e = reinterpret_cast<float*>(ema_ptrs[t]) + off;
+    const float* __restrict__ s = reinterpret_cast<const float*>(src_ptrs[t]) + off;
+    long long n = numels[t] - off;
+    if (n > chunk) n = chunk;
+    // kUnroll elements per thread and pass, all loaded before any is stored: one load pair per thread in flight
+    // leaves a 65536-element chunk latency-bound
+    constexpr int kUnroll = 8;
+    for (long long i0 = threadIdx.x; i0 < n; i0 += kUnroll * blockDim.x) {
+        float ev[kUnroll], sv[kUnroll];
+#pragma unroll
+        for (int j = 0; j < kUnroll; ++j) {
+            const long long i = i0 + j * blockDim.x;
+            if (i < n) {
+                ev[j] = e[i];
+                sv[j] = __ldg(s + i);
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < kUnroll; ++j) {
+            const long long i = i0 + j * blockDim.x;
+            if (i < n) e[i] = __fsub_rn(ev[j], __fmul_rn(w, __fsub_rn(ev[j], sv[j])));
+        }
+    }
+}
+
 }  // namespace effdet
 
 using namespace effdet;
@@ -210,4 +260,20 @@ extern "C" int effdet_multi_clip_adamw_dev(const uint64_t* p_ptrs, const uint64_
         reinterpret_cast<const long long*>(numels), chunk_tensor, reinterpret_cast<const long long*>(chunk_off), chunk,
         norm_sq, max_norm, lr, reinterpret_cast<long long*>(step), gate, ticket, beta1, beta2, eps, weight_decay);
     return launch_status("multi_clip_adamw_dev_kernel");
+}
+
+extern "C" int effdet_multi_ema(const uint64_t* ema_ptrs, const uint64_t* src_ptrs, const int64_t* numels,
+                                const int32_t* chunk_tensor, const int64_t* chunk_off, int nchunks, int chunk,
+                                double decay, int ramp, int64_t* updates, const int32_t* gate, uint32_t* ticket,
+                                int device, effdet_stream_t stream) {
+    EFFDET_REQUIRE(ema_ptrs && src_ptrs && numels && chunk_tensor && chunk_off && updates && ticket && nchunks > 0 &&
+                       chunk > 0,
+                   "multi_ema: bad arguments");
+    EFFDET_REQUIRE(decay >= 0.0 && decay <= 1.0, "multi_ema: decay must lie in [0, 1] (got %g)", decay);
+    EFFDET_DEVICE(device);
+    multi_ema_kernel<<<nchunks, 256, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<const unsigned long long*>(ema_ptrs), reinterpret_cast<const unsigned long long*>(src_ptrs),
+        reinterpret_cast<const long long*>(numels), chunk_tensor, reinterpret_cast<const long long*>(chunk_off), chunk,
+        decay, ramp, reinterpret_cast<long long*>(updates), gate, ticket);
+    return launch_status("multi_ema_kernel");
 }

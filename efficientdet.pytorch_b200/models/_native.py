@@ -170,6 +170,7 @@ SIGNATURES = {
     'effdet_multi_clip_adamw': [_P] * 7 + [_INT, _INT, _P] + [_F] * 8 + [_INT] + _TAIL,
     'effdet_multi_accumulate': [_P] * 5 + [_INT, _INT] + [_P] * 3 + _TAIL,
     'effdet_multi_clip_adamw_dev': [_P] * 7 + [_INT, _INT, _P, _F] + [_P] * 4 + [ctypes.c_double] * 2 + [_F] * 2 + _TAIL,
+    'effdet_multi_ema': [_P] * 5 + [_INT, _INT, ctypes.c_double, _INT] + [_P] * 3 + _TAIL,
     'effdet_normalize_pad': [_P, _P, _P, _P, _P, _INT, _INT, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)] + _TAIL,
     'effdet_resize_normalize_pad': [_P] * 6 + [_INT] * 3 + [ctypes.POINTER(ctypes.c_double)] * 2 + _TAIL,
     'effdet_collate_annots': [_P, _P, _P, _P, _P, _P, _INT, _INT] + _TAIL,

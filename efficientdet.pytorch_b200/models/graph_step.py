@@ -64,7 +64,8 @@ clip + AdamW update, which also empties the accumulators.  The loop as a user wr
 
     opt = FusedClipAdamW(model.parameters(), lr=lr, max_norm=0.1)    # opt.load_state_dict(...) here, if resuming
     scheduler = torch.optim.lr_scheduler.ReduceLROnPlateau(opt, patience=3)
-    step = GraphedTrainStep(model, images_example, annotations_example, optimizer=opt)
+    ema = ModelEma(model)                                  # optional; ema.load_state_dict(...) here, if resuming
+    step = GraphedTrainStep(model, images_example, annotations_example, optimizer=opt, ema=ema)
     for epoch in range(num_epoch):
         opt.zero_grad()
         losses = []
@@ -73,7 +74,10 @@ clip + AdamW update, which also empties the accumulators.  The loop as a user wr
             losses.append(loss.clone())                    # stays on the device: no synchronisation per step
         losses = torch.stack(losses)
         scheduler.step(float(losses[losses != 0].mean()))  # the reference averages the non-skipped losses
-        torch.save({'optimizer': opt.state_dict(), ...})  # true step counts: one device read
+        if (epoch + 1) % 5 == 0:
+            evaluate(valid_dataset, ema.module)            # train.py validates every 5 epochs; here on the average
+        torch.save({'state_dict': model.state_dict(), 'ema': ema.state_dict(),
+                    'optimizer': opt.state_dict(), ...})  # true step and EMA counts: one device read each
 
 The step counters and learning rates live in device memory: each call writes the `update` flag, and the lr of any
 param group whose `group['lr']` changed, into their device scalars before the replay (launches, no synchronisation),
@@ -82,6 +86,13 @@ raises.  Building the step leaves parameters, moments and step counts untouched:
 only.  Under DDP every call must update (`update=True`); gradient accumulation across DDP micro-steps is not
 supported.  Any other optimizer has its `step()` captured as is (the warm-up then runs it too) and allows
 `update=True` only.
+
+With `ema=ModelEma(model)` (models/ema.py) the captured region ends with one effdet_multi_ema launch after the
+optimizer's: the moving average of the weights advances exactly when the weights do.  With FusedClipAdamW it reads
+the optimizer's gate, so accumulation micro-steps and zero-loss batches leave the average and its counter untouched;
+with any other optimizer every replay updates it.  ema= needs an optimizer in the graph.  Building the step changes no
+averaged value, and every call bumps the versions of ema.module's averaged tensors (host-only work), so eager use of
+ema.module between replays (detect_batch, evaluate, a GraphedDetect built on it) derives its packed weights afresh.
 
 With an optimizer in the graph the packed-weight / folded-BN derivations are captured as well: they re-run on every
 replay because the weights change without Python seeing it.  For the same reason, eager use of the model between
@@ -101,7 +112,11 @@ class GraphedTrainStep:
     init_process_group, the DDP wrapper CONSTRUCTED inside a side-stream context, >= 11 eager warm-up iterations);
     gradients then have to flow through DDP's AccumulateGrad hooks, so the captured step calls loss.backward()."""
 
-    def __init__(self, model, images, annotations=None, optimizer=None, warmup=3, max_annotations=None, max_bytes=None):
+    def __init__(self, model, images, annotations=None, optimizer=None, warmup=3, max_annotations=None, max_bytes=None,
+                 ema=None):
+        if ema is not None and optimizer is None:
+            raise _ops.N.EffdetNativeError('GraphedTrainStep: ema= needs an optimizer in the graph; without one the '
+                                           'replays never change the weights it averages')
         self.raw = None
         if isinstance(images, pipeline.RawBatch):
             images = self._init_raw(model, images, annotations, max_annotations, max_bytes)
@@ -115,6 +130,8 @@ class GraphedTrainStep:
         self.model = model
         self.optimizer = optimizer
         self.fused = isinstance(optimizer, FusedClipAdamW)
+        self.ema = ema
+        self._ema_table = None if ema is None else ema._table(model)
         self.static_images = images.clone()
         self.static_counts = None
         if self.raw is not None:
@@ -255,6 +272,8 @@ class GraphedTrainStep:
                 self.optimizer._graph_launch({p: p.grad for p in params}, loss)
         elif self.optimizer is not None:
             self.optimizer.step()
+        if capture and self.ema is not None:                         # the warm-up leaves the EMA untouched too
+            self.ema._launch(self._ema_table, self.optimizer._graph['gate'] if self.fused else None)
         return loss.detach()
 
     def _check_batch(self, images, annotations):
@@ -317,6 +336,8 @@ class GraphedTrainStep:
             self.static_images.copy_(images, non_blocking=True)
             self.static_annots.copy_(annotations, non_blocking=True)
         self.graph.replay()
+        if self.ema is not None:
+            self.ema._bump_versions()
         return self.static_loss
 
 

@@ -483,6 +483,23 @@ int effdet_multi_clip_adamw_dev(const uint64_t* p_ptrs, const uint64_t* g_ptrs, 
                                 const int64_t* chunk_off, int nchunks, int chunk, const float* norm_sq, float max_norm,
                                 const float* lr, int64_t* step, const int32_t* gate, uint32_t* ticket, double beta1,
                                 double beta2, float eps, float weight_decay, int device, effdet_stream_t stream);
+/* Exponential moving average of the weights (Tan et al., EfficientDet section 5.1), over the same chunk tables:
+ * ema_ptrs[t] the averaged fp32 tensors, src_ptrs[t] the model's, one CTA per chunk.
+ *   gate      : gate[0] == 0 (the gate effdet_multi_accumulate writes): returns and writes nothing, not even the
+ *               counter.  gate NULL: every launch updates.
+ *   updates   : int64 counter; this launch is update k = updates[0] + 1, and advances updates[0] by exactly one.
+ *   ticket    : one zero-initialised uint32 that the launch returns to zero (every CTA reads the counter before it
+ *               takes a ticket; the last one advances it); launches sharing it must be stream-ordered.
+ *   decay     : d = ramp ? min(decay, (1 + k) / (10 + k)) : decay in fp64 -- TF's ExponentialMovingAverage(decay,
+ *               num_updates=k) -- then w = (float)(1 - d), rounded once.
+ *   element   : e = e - w * (e - s) in fp32, each operation rounded on its own (__fsub_rn / __fmul_rn, no FMA):
+ *               TF's assign_moving_average, variable - (variable - value) * (1 - decay).
+ * Refused (-1, message naming multi_ema): a NULL table, counter or ticket, nchunks < 1, chunk < 1, decay outside
+ * [0, 1]. */
+int effdet_multi_ema(const uint64_t* ema_ptrs, const uint64_t* src_ptrs, const int64_t* numels,
+                     const int32_t* chunk_tensor, const int64_t* chunk_off, int nchunks, int chunk, double decay,
+                     int ramp, int64_t* updates, const int32_t* gate, uint32_t* ticket, int device,
+                     effdet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) rank 2: the step BEFORE the hot path, on the device.  Normalizer + Augmenter (horizontal flip) + zero pad
